@@ -30,6 +30,7 @@ GMSM_HD void test_op_sizes(int op, int* wa, int* wb, int* wo) {
     case 10: *wa = 4 * FW; *wb = 0; *wo = 4 * FW; break;
     case 11: *wa = 4 * FW; *wb = 0; *wo = 2 * FW; break;
     case 12: *wa = G::Fr::N; *wb = 0; *wo = G::Fr::N; break;
+    case 13: *wa = 2 * FW; *wb = 2 * FW; *wo = FW; break;
     default: *wa = *wb = *wo = 0;
   }
 }
@@ -58,6 +59,8 @@ GMSM_HD void test_op_one(int op, const uint32_t* a, const uint32_t* b, uint32_t*
     case 10: wr(o, xyzz_double(rd<XYZZ<F>>(a))); break;
     case 11: wr(o, jac_to_affine(xyzz_to_jac(rd<XYZZ<F>>(a)))); break;
     case 12: wr(o, fp_from_mont(rd<typename G::Fr>(a))); break;
+    // the fused sum of products of the point formulas: fp_dot2 (G1), fp_dot4 or two fused Fp2 products (G2)
+    case 13: wr(o, f_dot2(rd<F>(a), rd<F>(b), rd<F>(a + G::F::N), rd<F>(b + G::F::N))); break;
     default: break;
   }
 }

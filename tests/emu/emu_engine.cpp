@@ -372,6 +372,33 @@ extern "C" int EMU_CAT(emu_batch_scalar_mul_, EMU_GROUP)(const void* base, const
 
 extern "C" void EMU_CAT(emu_set_block_order_, EMU_GROUP)(unsigned order) { emu_block_order = order; }
 
+// K1 alone: the digits k_digits_hist writes for the scalars (digits[j*n + i], W = ceil(fr.Bits / c) rows), in the plain
+// (rank_mode = 0) or the rank mode (1, warp collectives: cooperative launcher).  Returns 10 if the histogram does not
+// count exactly the non-zero digits.
+extern "C" int EMU_CAT(emu_digits_, EMU_GROUP)(const void* scalars, size_t n, int c, int rank_mode, uint32_t* digits_out) {
+  if (c < 2 || c > 24) return 1;
+  if (n == 0) return 0;
+  const WindowPlan p = make_plan(EmuG::FrParams::BITS, c);
+  const size_t nbp = (size_t)p.nb_total + 1;
+  std::vector<uint32_t> hist(nbp + 8, 0), ranks(n * (size_t)p.nwin + 16, 0xFFFFFFFFu);
+  hist[nbp + 4] = rank_mode ? 1u : 0u;
+  const auto* s = reinterpret_cast<const typename EmuG::Fr*>(scalars);
+  const dim3 grid(std::min<unsigned>(nblk(n, 256), GMSM_NUM_SMS * 16u));
+  if (rank_mode)
+    emu_launch_coop(k_digits_hist<EmuG>, grid, 256u, s, (uint32_t)n, p.c, p.nwin, p.nb, digits_out, ranks.data(), hist.data(),
+                    (const uint32_t*)(hist.data() + nbp + 4));
+  else
+    emu_launch(k_digits_hist<EmuG>, grid, 256u, s, (uint32_t)n, p.c, p.nwin, p.nb, digits_out, ranks.data(), hist.data(),
+               (const uint32_t*)(hist.data() + nbp + 4));
+  std::vector<uint32_t> want(nbp, 0);
+  for (int j = 0; j < p.nwin; j++)
+    for (size_t i = 0; i < n; i++)
+      if (const uint32_t code = digits_out[(size_t)j * n + i]) want[(size_t)j * p.nb + code_bucket(code)]++;
+  for (size_t b = 0; b < nbp; b++)
+    if (hist[b] != want[b]) return 10;
+  return 0;
+}
+
 // one rank's window partials (W x xyzz, or 1 in window-table mode), and the combine over ranks
 extern "C" int EMU_CAT(emu_window_sums_, EMU_GROUP)(const void* points, const void* scalars, size_t n, int c, int tables, uint32_t K, void* out_partials) {
   Opts o{c, tables, K, 4, 16, 32, 3, 1, 1, out_partials, 0};

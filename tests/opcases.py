@@ -8,7 +8,7 @@ import numpy as np
 from oracle import oracle as O
 
 OPS = dict(FMUL=0, FADD=1, FSUB=2, FSQR=3, FNEG=4, FDBL=5, FINV=6, ADD_MIXED=7, SUB_MIXED=8, ADD=9, DOUBLE=10, TO_AFFINE=11,
-           FR_FROM_MONT=12)
+           FR_FROM_MONT=12, FDOT2=13)
 
 
 def u32(a):
