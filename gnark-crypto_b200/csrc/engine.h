@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <cstdint>
 #include <mutex>
+#include <string>
 
 #include "../../include/gmsm.h"
 #include "groups.cuh"
@@ -46,9 +47,14 @@ struct gmsm_ctx {
   int table_passes = 0;   // bucket-range passes of the shared scatter (0 = from the entry count; GMSM_TABLE_PASSES)
   int red_windows() const { return shared ? 1 : plan.nwin; }   // partials per call
   // chunking
-  uint32_t K2 = 16;
+  uint32_t acc_K = 0;       // accumulate chunk length forced by GMSM_ACC_K (0 = pick_K)
+  uint32_t K2 = 16;         // items per thread of the later carry levels (GMSM_K2)
   uint32_t K2_first = 4;    // items per thread of the first carry level (GMSM_K2_FIRST): 4x the threads for the level that
                             // holds nearly all the carry additions (faster at bn254 G1 2^24)
+  int k1_mode = -1;         // counting-sort mode forced by GMSM_K1_MODE: 0 plain, 1 rank, -1 = chosen per call by k_skew_probe
+  // the GMSM_* experiment knobs this context was built under (knob_signature() in gmsm.cu): the host entry points keep a
+  // context between calls and build a new one when the environment no longer matches
+  std::string knobs;
   uint32_t seg_L = 32, seg_S = 0;
   // lane-parallel tail (quad.cuh): one QUAD of lanes per chain instead of one thread.  Slower than the serial form for the
   // 8- and 12-limb groups, so it is OFF unless GMSM_QUAD=1 asks for it

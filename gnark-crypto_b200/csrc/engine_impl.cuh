@@ -38,9 +38,14 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
   CK(cudaMemsetAsync(c->hist, 0, (nbp + 8) * 4, st));
   {
     unsigned blocks = std::min<unsigned>(nblk(n, 256), GMSM_NUM_SMS * 16u);
-    k_skew_probe<G><<<PROBE_BLOCKS, 256, 0, st>>>(scalars, n32, p.c, p.nwin, c->hist + nbp + 4);    // flag lives in the pad of hist[] (just cleared)
+    // the mode flag lives in the pad of hist[] (just cleared: plain); GMSM_K1_MODE forces it instead of sampling the scalars
+    if (c->k1_mode < 0) {
+      k_skew_probe<G><<<PROBE_BLOCKS, 256, 0, st>>>(scalars, n32, p.c, p.nwin, c->hist + nbp + 4);
+      launches++;
+    } else if (c->k1_mode == 1) {
+      CK(cudaMemsetAsync(c->hist + nbp + 4, 1, 1, st));   // little-endian word 1
+    }
     k_digits_hist<G><<<blocks, 256, 0, st>>>(scalars, n32, p.c, p.nwin, c->shared ? 0u : p.nb, c->digits, c->ranks, c->hist, c->hist + nbp + 4);
-    launches++;
     launches++;
     LAUNCH_CHECK();
   }
@@ -173,7 +178,7 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
     mark(4);
   } else {
   // K2: accumulate
-    const uint32_t K = pick_K(n, p.nwin);
+    const uint32_t K = c->acc_K ? c->acc_K : pick_K(n, p.nwin);
     const size_t nchunks = (n * (size_t)p.nwin + K - 1) / K;
     if (nchunks > c->max_chunks) return set_err(GMSM_EINVAL, "internal: chunk bound exceeded (%zu > %zu)", nchunks, c->max_chunks);
     CK(cudaMemsetAsync(buckets, 0, (size_t)p.nb_total * sizeof(X), st));

@@ -191,6 +191,20 @@ static int choose_c_tables(int fr_bits, size_t n) {
 // ------------------------------------------------------------------------------------------
 // context
 // ------------------------------------------------------------------------------------------
+// The experiment knobs a context reads once, when it is created.  Their values as a string: a session's context built under
+// other values is rebuilt (pipeline_run), so that changing a knob between two host calls takes effect on the second one.
+static std::string knob_signature() {
+  static const char* const names[] = {"GMSM_AFFINE", "GMSM_QUAD", "GMSM_QUAD_MAX", "GMSM_SPLIT_W", "GMSM_TABLE_PASSES",
+                                      "GMSM_K2_FIRST", "GMSM_K2", "GMSM_SEG_L", "GMSM_TABLE_SEG_L", "GMSM_ACC_K", "GMSM_K1_MODE"};
+  std::string s;
+  for (const char* nm : names) {
+    const char* e = getenv(nm);
+    s += e ? e : "-";   // unset is distinct from every value
+    s += '\x1f';
+  }
+  return s;
+}
+
 static int ctx_alloc(gmsm_ctx* c) {
   const WindowPlan& p = c->plan;
   const size_t xyzz = 16u * c->ci.coord_words;
@@ -206,10 +220,13 @@ static int ctx_alloc(gmsm_ctx* c) {
   CK(dmalloc(&c->buckets, (size_t)p.nb_total * xyzz, &acc));
   // chunks(n) = ceil(n*W / K(n)) <= max(GMSM_NUM_SMS*512*8 (+slack), ceil(max_n*W/128))  -- see pick_K
   size_t mc = std::max<size_t>(700000, (ent + 127) / 128 + 1);
+  // GMSM_ACC_K: every call cuts its n*W entries into chunks of exactly acc_K
+  if (c->acc_K) mc = std::max<size_t>(mc, (ent + c->acc_K - 1) / c->acc_K + 1);
   c->max_chunks = mc;
   CK(dmalloc(&c->carries[0], mc * xyzz, &acc));
   CK(dmalloc(&c->carry_ids[0], (mc + 8) * 4, &acc));
   if (const char* e = getenv("GMSM_K2_FIRST")) { int v = atoi(e); if (v >= 2 && v <= 64) c->K2_first = (uint32_t)v; }
+  if (const char* e = getenv("GMSM_K2")) { int v = atoi(e); if (v >= 2 && v <= 64) c->K2 = (uint32_t)v; }
   const uint32_t k2min = std::min(c->K2, c->K2_first);
   size_t mc2 = (mc + k2min - 1) / k2min;
   CK(dmalloc(&c->carries[1], mc2 * xyzz, &acc));
@@ -334,6 +351,14 @@ static gmsm_ctx* ctx_create_ex(gmsm_curve_t curve, size_t max_n, int c, int devi
   if (const char* e = getenv("GMSM_QUAD")) { ctx->quad_mode = atoi(e); ctx->quad_max_items = (size_t)1 << 40; }
   if (const char* e = getenv("GMSM_QUAD_MAX")) { long v = atol(e); if (v >= 0) ctx->quad_max_items = (size_t)v; }
   if (const char* e = getenv("GMSM_SPLIT_W")) { int v = atoi(e); if (v >= 1 && v <= 64) ctx->split_w = ctx->split_tab = v; }
+  // shapes the heuristics never pick (tests, experiments): the accumulate chunk length, and the counting-sort mode without
+  // the sampling pass (GMSM_K1_MODE=plain|rank)
+  if (const char* e = getenv("GMSM_ACC_K")) { int v = atoi(e); if (v >= 1 && v <= 256) ctx->acc_K = (uint32_t)v; }
+  if (const char* e = getenv("GMSM_K1_MODE")) {
+    if (!strcmp(e, "plain")) ctx->k1_mode = 0;
+    else if (!strcmp(e, "rank")) ctx->k1_mode = 1;
+  }
+  ctx->knobs = knob_signature();
   ctx->plan = make_plan(ci.fr_bits, c);
   if (shared) ctx->plan.nb_total = std::max(ctx->plan.nb, ctx->plan.nb_last);   // one bucket set for all windows
   if ((double)max_n * ctx->plan.nwin >= 4294967000.0) {
@@ -729,7 +754,8 @@ static int pipeline_run(Pipeline& P, void* d_points, const uint64_t* h_points, c
   }
   // window width from the TOTAL size (all batches share one bucket array); workspace sized for one batch
   const int c = P.tables ? P.tab_c : (c_force ? c_force : choose_c_for(P.curve, ci.fr_bits, n));
-  if (!P.ctx || P.ctx->max_n < nc || P.ctx->max_n > 4 * nc + 1024 || P.ctx->plan.c != c || P.ctx->shared != P.tables) {
+  if (!P.ctx || P.ctx->max_n < nc || P.ctx->max_n > 4 * nc + 1024 || P.ctx->plan.c != c || P.ctx->shared != P.tables ||
+      P.ctx->knobs != knob_signature()) {
     if (P.ctx) { gmsm_ctx_destroy(P.ctx); P.ctx = nullptr; }
     P.ctx = ctx_create_ex((gmsm_curve_t)P.curve, nc, c, P.device, P.tables);
     if (!P.ctx) return GMSM_ECUDA;
@@ -1061,7 +1087,8 @@ extern "C" int gmsm_bases_multiexp_device(gmsm_bases_t* b, size_t offset, const 
   Pipeline& P = sh.pipe;
   CK(cudaSetDevice(P.device));
   const int c = P.tables ? P.tab_c : choose_c_for(P.curve, ci.fr_bits, n);
-  if (!P.ctx || P.ctx->max_n < n || P.ctx->max_n > 4 * n + 1024 || P.ctx->plan.c != c || P.ctx->shared != P.tables) {
+  if (!P.ctx || P.ctx->max_n < n || P.ctx->max_n > 4 * n + 1024 || P.ctx->plan.c != c || P.ctx->shared != P.tables ||
+      P.ctx->knobs != knob_signature()) {
     if (P.ctx) { gmsm_ctx_destroy(P.ctx); P.ctx = nullptr; }
     P.ctx = ctx_create_ex((gmsm_curve_t)P.curve, n, c, P.device, P.tables);
     if (!P.ctx) return GMSM_ECUDA;

@@ -146,12 +146,16 @@ def test_device_level_calls_on_one_context_from_two_streams():
     eng.close()
 
 
-@pytest.mark.parametrize("g,n", [("bn254_g1", 50000), ("bls12381_g1", 20000), ("bn254_g2", 12000), ("bls12381_g2", 6000)])
+@pytest.mark.parametrize("g,n", [("bn254_g1", 50000), ("bls12381_g1", 20000), ("bn254_g2", 12000), ("bls12381_g2", 6000),
+                                 ("bls12377_g1", 20000), ("bls12377_g2", 6000), ("secp256k1_g1", 50000), ("bw6761_g1", 4000),
+                                 ("bw6761_g2", 4000), ("bls24315_g1", 30000), ("bls24317_g1", 30000), ("bw6633_g1", 5000),
+                                 ("bw6633_g2", 5000)])
 @pytest.mark.parametrize("quad", ["0", "1"])
 def test_tail_kernels_serial_and_lane_parallel(g, n, quad, monkeypatch):
     """the carry join / bucket reduction / group sums in their one-thread-per-chain and one-quad-per-chain forms (csrc/quad.cuh)
     are both exact, at several widths, with the cross-test ingredients and with every scalar equal (one bucket per window
-    spans all the chunks: the carry levels do the work)"""
+    spans all the chunks: the carry levels do the work).  All thirteen groups; GMSM_QUAD=0 is the serial form also for the
+    bw6 groups, whose default is lane-parallel"""
     monkeypatch.setenv("GMSM_QUAD", quad)
     pkg = _pkg()
     pts, s = make_inputs(g, n, 17)

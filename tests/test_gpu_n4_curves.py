@@ -29,6 +29,14 @@ def _pkg():
     return pkg
 
 
+@pytest.fixture(params=["affine", "xyzz"])
+def accumulate_mode(request, monkeypatch):
+    """both bucket-accumulation paths: the extended-Jacobian segmented reduction (the default) and the batch-affine tree
+    (GMSM_AFFINE=1)"""
+    monkeypatch.setenv("GMSM_AFFINE", "1" if request.param == "affine" else "0")
+    return request.param
+
+
 def _jac_cls(g):
     A1, J1, A2, J2 = _pkg().curve_package(g.split("_")[0])
     return (J1, A1) if g.endswith("g1") else (J2, A2)
@@ -63,9 +71,9 @@ def test_sizes_of_the_new_curves():
                                      ("bls24317_g1", 1000, [3, 8, 15, 16, 17]),                      # 255 = 15 * 17: last windows of c + 1 bits
                                      ("bw6633_g1", 600, [4, 5, 6, 7, 8, 9, 12, 15, 16, 18]),         # 315 = 5 * 63 = 7 * 45 = 9 * 35 = 15 * 21
                                      ("bw6633_g2", 400, [6, 12, 16])])
-def test_window_sizes_agree_with_oracle(g, n, cs):
+def test_window_sizes_agree_with_oracle(g, n, cs, accumulate_mode):
     """the widths the reference implements for the curve (multiexp.go:77) and the wider ones the GPU model may pick; inputs
-    with the cross-test ingredients (infinities, duplicates, P / -P, zero scalars)"""
+    with the cross-test ingredients (infinities, duplicates, P / -P, zero scalars); both accumulation paths"""
     pts, s = make_inputs(g, n, 4321)
     want, _, used_c, _ = cref.msm(g, pts, s, c=0, nthreads=4)
     assert used_c in O.IMPLEMENTED_CS[g]
