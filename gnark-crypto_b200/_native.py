@@ -24,7 +24,7 @@ SYMBOLS = [
     "gmsm_bases_precompute", "gmsm_bases_table_bits", "gmsm_ctx_create_tables", "gmsm_tables_build_device", "gmsm_ctx_msm_tables_device",
     "gmsm_ctx_create", "gmsm_ctx_destroy", "gmsm_ctx_window_bits", "gmsm_ctx_num_windows", "gmsm_ctx_workspace_bytes",
     "gmsm_ctx_last_launches", "gmsm_ctx_msm_device", "gmsm_ctx_window_sums_device", "gmsm_ctx_finalize_device",
-    "gmsm_ctx_set_profiling", "gmsm_ctx_last_stage_ms", "gmsm_generate_multiples_device", "gmsm_batch_scalar_mul", "gmsm_g1_decode", "gmsm_g1_decode_device", "gmsm_fft_domain_create", "gmsm_fft_domain_free", "gmsm_fft_domain_cardinality",
+    "gmsm_ctx_set_profiling", "gmsm_ctx_last_stage_ms", "gmsm_generate_multiples_device", "gmsm_batch_scalar_mul", "gmsm_g1_decode", "gmsm_g1_decode_device", "gmsm_fft_fr_bytes", "gmsm_fft_domain_create", "gmsm_fft_domain_free", "gmsm_fft_domain_cardinality",
     "gmsm_fft_domain_constants", "gmsm_fft", "gmsm_fft_inverse", "gmsm_fft_device", "gmsm_fft_bit_reverse_device", "gmsm_test_op", "gmsm_test_digits",
 ]
 
@@ -89,6 +89,8 @@ def lib() -> ctypes.CDLL:
     L.gmsm_batch_scalar_mul.argtypes = [i32, vp, vp, sz, vp]
     L.gmsm_g1_decode.argtypes = [i32, vp, sz, i32, i32, vp]
     L.gmsm_g1_decode_device.argtypes = [i32, vp, sz, i32, i32, vp, vp, vp]
+    L.gmsm_fft_fr_bytes.restype = sz
+    L.gmsm_fft_fr_bytes.argtypes = [i32]
     L.gmsm_fft_domain_create.restype = vp
     L.gmsm_fft_domain_create.argtypes = [i32, ctypes.c_uint64, vp, i32]
     L.gmsm_fft_domain_free.argtypes = [vp]

@@ -2,150 +2,24 @@
 // gnark-crypto's standard WriteTo format and the resident bases of the MSM engine.
 //
 // Replaces (reference): G1Affine.SetBytes / setBytes without the subgroup check (ecc/bn254/marshal.go:858-950,
-// ecc/bls12-381/marshal.go:886-1000; the Decoder's NoSubgroupChecks path, marshal.go:52-60, which also splits the work in
-// "read X" and "unsafeComputeY", :952-990), fp.Element.SetBytesCanonical (fp/element.go:905-925), fp.Sqrt for q = 3 mod 4
-// (fp/element.go:1142-1153: y = x^((q+1)/4), checked by squaring), LexicographicallyLargest (fp/element.go:282-296).
+// ecc/bls12-381/marshal.go:886-1000, and the same code of bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761; the Decoder's
+// NoSubgroupChecks path, marshal.go:52-60, which also splits the work in "read X" and "unsafeComputeY", :952-990),
+// fp.Element.SetBytesCanonical (fp/element.go:905-925), fp.Sqrt (fp/element.go:1142-1153 for q = 3 mod 4: y = x^((q+1)/4);
+// here Tonelli-Shanks for every q, which is that same power when q = 3 mod 4; checked by squaring), LexicographicallyLargest
+// (fp/element.go:282-296).
 // Wire format: big-endian X (|| Y), canonical (non-Montgomery) values, flag bits in the most significant byte:
 //   bn254 (two spare bits, marshal.go:25-31):      00 uncompressed | 10 compressed, smallest y | 11 largest y | 01 infinity
-//   bls12-381 / bls12-377 (three bits, :27-34):   000 uncompressed | 010 uncompressed infinity | 100 / 101 compressed | 110 infinity
-// One thread per point; results are the reference's in-memory G1Affine (Montgomery limbs, infinity = zeroes).
+//   bls12-381 / bls12-377 / bls24-315 / bls24-317 / bw6-633 / bw6-761 (three bits, :27-34):
+//                                                 000 uncompressed | 010 uncompressed infinity | 100 / 101 compressed | 110 infinity
+// One thread per point (decode_kernels.cuh); results are the reference's in-memory G1Affine (Montgomery limbs, infinity = zeroes).
 #include <cuda_runtime.h>
 
 #include <cstdint>
 #include <cstring>
 
 #include "engine.h"
-#include "kernels.cuh"
 
-namespace gmsm {
-
-enum { DEC_OK = 0, DEC_BAD_INFINITY = 1, DEC_BAD_ELEMENT = 2, DEC_NO_SQRT = 3, DEC_NOT_ON_CURVE = 4, DEC_BAD_FLAGS = 5 };
-
-template <class P>
-struct WireFlags {
-  static constexpr int SPARE = 32 * P::N - P::BITS;
-  static constexpr bool THREE = SPARE >= 3;
-  static constexpr uint32_t MASK = THREE ? (0b111u << 5) : (0b11u << 6);
-  static constexpr uint32_t UNC = 0;
-  static constexpr uint32_t UNC_INF = THREE ? (0b010u << 5) : 0xFFFFu;     // (none for bn254)
-  static constexpr uint32_t SMALL = THREE ? (0b100u << 5) : (0b10u << 6);
-  static constexpr uint32_t LARGE = THREE ? (0b101u << 5) : (0b11u << 6);
-  static constexpr uint32_t INF = THREE ? (0b110u << 5) : (0b01u << 6);
-};
-
-// big-endian bytes -> little-endian 32-bit limbs (canonical integer), top byte masked with `keep`
-template <class P>
-GMSM_D Fp<P> read_be(const uint8_t* b, uint32_t keep) {
-  constexpr int N = P::N;
-  Fp<P> r;
-#pragma unroll
-  for (int k = 0; k < N; k++) {
-    const uint8_t* q = b + 4 * (N - 1 - k);
-    uint32_t v = ((uint32_t)q[0] << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | (uint32_t)q[3];
-    if (k == N - 1) v &= (keep << 24) | 0x00FFFFFFu;
-    r.l[k] = v;
-  }
-  return r;
-}
-template <class P>
-GMSM_D bool below_modulus(const Fp<P>& a) {   // smallerThanModulus, fp/element.go:347-349
-  for (int i = P::N - 1; i >= 0; i--) {
-    if (a.l[i] < P::mod(i)) return true;
-    if (a.l[i] > P::mod(i)) return false;
-  }
-  return false;
-}
-// canonical value > (q - 1) / 2  <=>  2 * value > q - 1  <=>  2 * value >= q + 1 ... evaluated as value >= (q + 1) / 2
-template <class P>
-GMSM_D bool lexicographically_largest(const Fp<P>& y_mont) {
-  const Fp<P> y = fp_from_mont(y_mont);
-  // h = (q + 1) / 2 (q odd): q >> 1, plus one
-  uint32_t h[P::N];
-#pragma unroll
-  for (int i = 0; i < P::N; i++) h[i] = (P::mod(i) >> 1) | ((i + 1 < P::N ? P::mod(i + 1) : 0u) << 31);
-  uint32_t carry = 1;
-#pragma unroll
-  for (int i = 0; i < P::N; i++) { const uint32_t s = h[i] + carry; carry = (s < carry) ? 1u : 0u; h[i] = s; }
-  for (int i = P::N - 1; i >= 0; i--) {
-    if (y.l[i] > h[i]) return true;
-    if (y.l[i] < h[i]) return false;
-  }
-  return true;
-}
-// x^((q+1)/4) for q = 3 mod 4
-template <class P>
-GMSM_D Fp<P> sqrt_candidate(const Fp<P>& x) {
-  uint32_t e[P::N];   // (q + 1) >> 2; q + 1 does not overflow the limbs (spare top bits)
-  uint32_t carry = 1;
-#pragma unroll
-  for (int i = 0; i < P::N; i++) { const uint32_t s = P::mod(i) + carry; carry = (s < carry) ? 1u : 0u; e[i] = s; }
-#pragma unroll
-  for (int i = 0; i < P::N; i++) e[i] = (e[i] >> 2) | ((i + 1 < P::N ? e[i + 1] : 0u) << 30);
-  Fp<P> acc = Fp<P>::one();
-  bool started = false;
-  for (int i = 32 * P::N - 1; i >= 0; i--) {
-    if (started) acc = fp_sqr(acc);
-    if ((e[i >> 5] >> (i & 31)) & 1u) {
-      acc = started ? fp_mul(acc, x) : x;
-      started = true;
-    }
-  }
-  return acc;
-}
-
-template <class P>
-__global__ void __launch_bounds__(128)
-k_g1_decode(const uint8_t* __restrict__ bytes, uint32_t n, int raw, int check_curve, uint32_t b_small, Affine<Fp<P>>* __restrict__ out,
-            unsigned long long* __restrict__ first_error) {
-  using F = Fp<P>;
-  using W = WireFlags<P>;
-  constexpr int NB = 4 * P::N;
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint8_t* b = bytes + (size_t)i * (raw ? 2 * NB : NB);
-  const uint32_t m = b[0] & W::MASK;
-  int err = DEC_OK;
-  Affine<F> pt = Affine<F>::inf();
-  const bool is_inf = (m == W::INF) || (m == W::UNC_INF);
-  if (is_inf) {
-    const int len = (m == W::UNC_INF) ? 2 * NB : NB;
-    uint32_t any = b[0] & ~W::MASK & 0xFFu;
-    for (int k = 1; k < len; k++) any |= b[k];
-    if (any) err = DEC_BAD_INFINITY;
-  } else if ((raw && m != W::UNC) || (!raw && m != W::SMALL && m != W::LARGE)) {
-    err = DEC_BAD_FLAGS;     // a stream is homogeneous: raw = 1 holds uncompressed points, raw = 0 compressed ones
-  } else {
-    const F xc = read_be<P>(b, ~W::MASK & 0xFFu);
-    if (!below_modulus(xc)) err = DEC_BAD_ELEMENT;
-    const F X = fp_to_mont(xc);
-    F bm = F::zero();
-    bm.l[0] = b_small;
-    bm = fp_to_mont(bm);
-    const F rhs = fp_add(fp_mul(fp_sqr(X), X), bm);       // x^3 + b   (marshal.go:925-927)
-    if (raw) {
-      const F yc = read_be<P>(b + NB, 0xFFu);
-      if (!below_modulus(yc)) err = DEC_BAD_ELEMENT;
-      const F Y = fp_to_mont(yc);
-      if (!err && check_curve && !(fp_sqr(Y) == rhs) && !(xc.is_zero() && yc.is_zero())) err = DEC_NOT_ON_CURVE;
-      pt.x = X;
-      pt.y = Y;
-    } else {
-      F Y = sqrt_candidate(rhs);
-      if (!err && !(fp_sqr(Y) == rhs)) err = DEC_NO_SQRT;       // fp.Sqrt returns nil, marshal.go:928-930
-      const bool largest = lexicographically_largest(Y);
-      if (largest != (m == W::LARGE)) Y = fp_neg(Y);            // marshal.go:932-942
-      pt.x = X;
-      pt.y = Y;
-    }
-  }
-  if (err) {
-    atomicMin(first_error, ((unsigned long long)i << 8) | (unsigned long long)err);
-    pt = Affine<F>::inf();
-  }
-  store_vec(out + i, pt);
-}
-
-}  // namespace gmsm
+#include "decode_kernels.cuh"
 
 using namespace gmsm;
 
@@ -161,8 +35,9 @@ static const char* dec_message(int code) {
 }
 
 template <class P>
-static int run_decode(const void* d_bytes, size_t n, int raw, int check, uint32_t b_small, void* d_out, unsigned long long* d_err, cudaStream_t st) {
-  k_g1_decode<P><<<nblk(n, 128), 128, 0, st>>>(reinterpret_cast<const uint8_t*>(d_bytes), (uint32_t)n, raw, check, b_small,
+static int run_decode(const void* d_bytes, size_t n, int raw, int check, const DecodeConsts<P>& kc, void* d_out, unsigned long long* d_err,
+                      cudaStream_t st) {
+  k_g1_decode<P><<<nblk(n, 128), 128, 0, st>>>(reinterpret_cast<const uint8_t*>(d_bytes), (uint32_t)n, raw, check, kc,
                                               reinterpret_cast<Affine<Fp<P>>*>(d_out), d_err);
   CK(cudaGetLastError());
   return GMSM_OK;
@@ -176,14 +51,11 @@ extern "C" int gmsm_g1_decode_device(gmsm_curve_t curve, const void* d_bytes, si
   if (n > 0xFFFFFF00ull) return set_err(GMSM_EINVAL, "n too large");
   CK(cudaMemsetAsync(d_first_error, 0xFF, 8, st));
   if (n == 0) return GMSM_OK;
-  switch (curve) {
-    case GMSM_BN254_G1: return run_decode<bn254_fp>(d_bytes, n, raw, check_on_curve, 3, d_points, (unsigned long long*)d_first_error, st);
-    case GMSM_BLS12381_G1: return run_decode<bls12381_fp>(d_bytes, n, raw, check_on_curve, 4, d_points, (unsigned long long*)d_first_error, st);
-    case GMSM_BLS12377_G1:
-      if (!raw) return set_err(GMSM_EINVAL, "bls12-377 compressed points need a Tonelli-Shanks square root (q = 1 mod 4): decode them on the host");
-      return run_decode<bls12377_fp>(d_bytes, n, raw, check_on_curve, 1, d_points, (unsigned long long*)d_first_error, st);
-    default: return set_err(GMSM_EINVAL, "gmsm_g1_decode: G1 groups only (curve id %d)", (int)curve);
-  }
+  const int rc = with_g1_decode_consts(curve, [&](const auto& kc) {
+    return run_decode(d_bytes, n, raw, check_on_curve, kc, d_points, (unsigned long long*)d_first_error, st);
+  });
+  if (rc < 0) return set_err(GMSM_EINVAL, "gmsm_g1_decode: G1 groups of the pairing curves only (curve id %d)", (int)curve);
+  return rc;
 }
 
 // host bytes -> host points (Go memory layout), n points of a homogeneous stream (raw = 1: RawBytes, 0: Bytes)

@@ -1,6 +1,7 @@
 // Next-row N3: radix-2 FFT over Fr on the GPU, behind gnark-crypto's fft.Domain interface.
 //
-// Replaces (reference tree; ecc/bls12-381/fr/fft is the same generated code with its own constants):
+// Replaces (reference tree; the fr/fft packages of bls12-381, bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761 are the same
+// generated code with their own constants):
 //   fft.NewDomain / Domain{Cardinality, CardinalityInv, Generator, GeneratorInv, FrMultiplicativeGen(Inv)}
 //                                                             ecc/bn254/fr/fft/domain.go:24-110
 //   fr.Generator(m) (2-adic root of unity, maxOrderRoot)      ecc/bn254/fr/generator.go:18-36
@@ -8,10 +9,10 @@
 //   option; FFTInverse scales by CardinalityInv)              ecc/bn254/fr/fft/fft.go:31-190, difFFT :195+, ditFFT :262+
 //   BitReverse                                                 ecc/bn254/fr/fft/bitreverse.go:17-42
 //
-// Data is the reference's []fr.Element image (4 x u64 Montgomery limbs).  Kernels: one launch per butterfly
+// Data is the reference's []fr.Element image (fr.Limbs u64 Montgomery limbs: 4; 5 for bw6-633, 6 for bw6-761).  Kernels: one launch per butterfly
 // stage for the strided stages, one shared-memory kernel for the last (DIF) / first (DIT) TILE_LOG stages,
 // twiddles w^j (j < n/2) precomputed per domain like the reference's Domain.twiddles; coset powers are
-// computed on the fly from u^(2^k).  HBM-bound streaming work: 32 B per element per pass.
+// computed on the fly from u^(2^k).  HBM-bound streaming work: fr.Bytes (32 / 40 / 48) per element per pass.
 #include <cuda_runtime.h>
 
 #include <cstdio>
@@ -57,13 +58,54 @@ const FrConsts FR_BN254 = {"1910321906792171394429139282769207003614565195732928
 const FrConsts FR_BLS12381 = {"10238227357739495823651030575849232062558860180284477541189508159991286009131", 32, 7};
 // ecc/bls12-377/fr/generator.go:23-24, fr/fft/domain.go:59
 const FrConsts FR_BLS12377 = {"8065159656716812877374967518403273466521432693661810619979959746626482506078", 47, 22};
+// ecc/{bls24-315,bls24-317,bw6-633,bw6-761}/fr/generator.go:23-24, fr/fft/domain.go:59.  Each root is
+// GeneratorFullMultiplicativeGroup^((r - 1) >> maxOrderRoot), of order exactly 2^maxOrderRoot.
+const FrConsts FR_BLS24315 = {"1792993287828780812362846131493071959406149719416102105453370749552622525216", 22, 7};
+const FrConsts FR_BLS24317 = {"16532287748948254263922689505213135976137839535221842169193829039521719560631", 60, 7};
+const FrConsts FR_BW6633 = {"4991787701895089137426454739366935169846548798279261157172811661565882460884369603588700158257", 20, 13};
+const FrConsts FR_BW6761 = {
+    "32863578547254505029601261939868325669770508939375122462904745766352256812585773382134936404344547323199885654433", 46, 15};
+
+const FrConsts* fr_consts(int field) {
+  switch (field) {
+    case GMSM_FR_BN254: return &FR_BN254;
+    case GMSM_FR_BLS12381: return &FR_BLS12381;
+    case GMSM_FR_BLS12377: return &FR_BLS12377;
+    case GMSM_FR_BLS24315: return &FR_BLS24315;
+    case GMSM_FR_BLS24317: return &FR_BLS24317;
+    case GMSM_FR_BW6633: return &FR_BW6633;
+    case GMSM_FR_BW6761: return &FR_BW6761;
+  }
+  return nullptr;
+}
+
+template <class P>
+struct FrTag {
+  using type = P;
+};
+// calls fn(FrTag<P>{}) with the Fp parameters of a scalar field id (checked by the caller)
+template <class Fn>
+int with_fr(int field, Fn&& fn) {
+  switch (field) {
+    case GMSM_FR_BN254: return fn(FrTag<bn254_fr>{});
+    case GMSM_FR_BLS12381: return fn(FrTag<bls12381_fr>{});
+    case GMSM_FR_BLS12377: return fn(FrTag<bls12377_fr>{});
+    case GMSM_FR_BLS24315: return fn(FrTag<bls24315_fr>{});
+    case GMSM_FR_BLS24317: return fn(FrTag<bls24317_fr>{});
+    case GMSM_FR_BW6633: return fn(FrTag<bw6633_fr>{});
+    case GMSM_FR_BW6761: return fn(FrTag<bw6761_fr>{});
+  }
+  return set_err(GMSM_EINVAL, "unknown scalar field %d", field);
+}
+constexpr int FR_MAX_WORDS = 6;   // u64 limbs of the widest scalar field (bw6-761)
 
 }  // namespace
 
 struct gmsm_fft_domain {
   int field = 0, device = 0, logn = 0;
+  int words = 0;                // u64 limbs per element (fr.Limbs); elements are 8 * words bytes
   uint64_t n = 0;
-  uint64_t consts[5][4] = {};   // Generator, GeneratorInv, CardinalityInv, FrMultiplicativeGen, FrMultiplicativeGenInv
+  uint64_t consts[5][FR_MAX_WORDS] = {};   // Generator, GeneratorInv, CardinalityInv, FrMultiplicativeGen, FrMultiplicativeGenInv
   void *d_tw = nullptr, *d_tw_inv = nullptr;       // w^j, w^-j for j < n/2
   void *d_pw = nullptr;                            // [0..63]: u^(2^k); [64..127]: u^-(2^k); [128..191]: scratch for twiddle builds
   void* d_buf = nullptr;                           // staging for the host entry points
@@ -76,11 +118,12 @@ static int domain_build(gmsm_fft_domain* d, const FrConsts& fc, const uint64_t* 
   F gen = host_pow2k(host_from_decimal<P>(fc.root), fc.max_order - d->logn);
   F gen_inv = fp_inv(gen);
   F card_inv = fp_inv(host_from_u64<P>(d->n));
+  static_assert(sizeof(F) <= sizeof(d->consts[0]), "consts row too small");
   F shift;
-  if (shift_mont) memcpy(shift.l, shift_mont, 32); else shift = host_from_u64<P>(fc.mult_gen);
+  if (shift_mont) memcpy(shift.l, shift_mont, sizeof(F)); else shift = host_from_u64<P>(fc.mult_gen);
   F shift_inv = fp_inv(shift);
-  memcpy(d->consts[0], gen.l, 32); memcpy(d->consts[1], gen_inv.l, 32); memcpy(d->consts[2], card_inv.l, 32);
-  memcpy(d->consts[3], shift.l, 32); memcpy(d->consts[4], shift_inv.l, 32);
+  memcpy(d->consts[0], gen.l, sizeof(F)); memcpy(d->consts[1], gen_inv.l, sizeof(F)); memcpy(d->consts[2], card_inv.l, sizeof(F));
+  memcpy(d->consts[3], shift.l, sizeof(F)); memcpy(d->consts[4], shift_inv.l, sizeof(F));
   F pw[192];
   F a = shift, b = shift_inv, g = gen, gi = gen_inv;
   for (int k = 0; k < 64; k++) { pw[k] = a; pw[64 + k] = b; a = fp_sqr(a); b = fp_sqr(b); }
@@ -130,7 +173,7 @@ static int run_fft(gmsm_fft_domain* d, void* d_a, int inverse, int decimation, i
   if (inverse) {
     // FFTInverse: scale by CardinalityInv, and on a coset by u^-i (DIT, natural output) or u^-bitrev(i) (DIF)
     F ci;
-    memcpy(ci.l, d->consts[2], 32);
+    memcpy(ci.l, d->consts[2], sizeof(F));
     k_fft_scale<P><<<grid(n), 256, 0, st>>>(a, n, d->logn, pw + 64, coset ? 1 : 0, decimation == 1 /*DIF*/, ci, 1);
   }
   CK(cudaGetLastError());
@@ -138,13 +181,14 @@ static int run_fft(gmsm_fft_domain* d, void* d_a, int inverse, int decimation, i
 }
 
 extern "C" gmsm_fft_domain_t* gmsm_fft_domain_create(int fr_field, uint64_t m, const uint64_t* shift, int device) {
-  if (fr_field < 0 || fr_field > 2) { set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field); return nullptr; }
+  const FrConsts* fcp = fr_consts(fr_field);
+  if (!fcp) { set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field); return nullptr; }
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev == 0) { set_err(GMSM_ENODEV, "no CUDA device (%s); this engine has no CPU fallback", cudaGetErrorString(e)); return nullptr; }
   if (device < 0 || device >= ndev) { set_err(GMSM_EINVAL, "device %d out of range", device); return nullptr; }
   cudaSetDevice(device);
-  const FrConsts& fc = fr_field == 0 ? FR_BN254 : (fr_field == 1 ? FR_BLS12381 : FR_BLS12377);
+  const FrConsts& fc = *fcp;
   uint64_t x = 1;
   int logn = 0;
   while (x < m) { x <<= 1; logn++; }   // ecc.NextPowerOfTwo(m)
@@ -154,9 +198,10 @@ extern "C" gmsm_fft_domain_t* gmsm_fft_domain_create(int fr_field, uint64_t m, c
   }
   gmsm_fft_domain* d = new gmsm_fft_domain();
   d->field = fr_field; d->device = device; d->n = x; d->logn = logn;
-  int rc = fr_field == 0 ? domain_build<bn254_fr>(d, fc, shift)
-                         : (fr_field == 1 ? domain_build<bls12381_fr>(d, fc, shift) : domain_build<bls12377_fr>(d, fc, shift));
-  if (rc == GMSM_OK && cudaMalloc(&d->d_buf, x * 32) != cudaSuccess) rc = set_err(GMSM_ENOMEM, "cudaMalloc(%llu) failed", (unsigned long long)(x * 32));
+  d->words = (int)(gmsm_fft_fr_bytes(fr_field) / 8);
+  int rc = with_fr(fr_field, [&](auto tag) { return domain_build<typename decltype(tag)::type>(d, fc, shift); });
+  const uint64_t buf_bytes = x * 8 * (uint64_t)d->words;
+  if (rc == GMSM_OK && cudaMalloc(&d->d_buf, buf_bytes) != cudaSuccess) rc = set_err(GMSM_ENOMEM, "cudaMalloc(%llu) failed", (unsigned long long)buf_bytes);
   if (rc != GMSM_OK) { cudaFree(d->d_tw); cudaFree(d->d_tw_inv); cudaFree(d->d_pw); cudaFree(d->d_buf); delete d; return nullptr; }
   return d;
 }
@@ -168,20 +213,27 @@ extern "C" void gmsm_fft_domain_free(gmsm_fft_domain_t* d) {
   delete d;
 }
 
+extern "C" size_t gmsm_fft_fr_bytes(int fr_field) {
+  switch (fr_field) {
+    case GMSM_FR_BN254: case GMSM_FR_BLS12381: case GMSM_FR_BLS12377: case GMSM_FR_BLS24315: case GMSM_FR_BLS24317: return 32;
+    case GMSM_FR_BW6633: return 40;
+    case GMSM_FR_BW6761: return 48;
+  }
+  return 0;
+}
+
 extern "C" uint64_t gmsm_fft_domain_cardinality(const gmsm_fft_domain_t* d) { return d ? d->n : 0; }
 
-extern "C" int gmsm_fft_domain_constants(const gmsm_fft_domain_t* d, uint64_t out[20]) {
+extern "C" int gmsm_fft_domain_constants(const gmsm_fft_domain_t* d, uint64_t* out) {
   if (!d) return set_err(GMSM_EINVAL, "null domain");
-  memcpy(out, d->consts, sizeof(d->consts));
+  for (int k = 0; k < 5; k++) memcpy(out + k * d->words, d->consts[k], 8 * (size_t)d->words);   // 5 x words limbs
   return GMSM_OK;
 }
 
 // unlocked dispatcher: callers hold d->mu
 static int fft_dispatch(gmsm_fft_domain_t* d, void* d_a, int inverse, int decimation, int coset, cudaStream_t st) {
   CK(cudaSetDevice(d->device));
-  if (d->field == 0) return run_fft<bn254_fr>(d, d_a, inverse, decimation, coset, st);
-  if (d->field == 1) return run_fft<bls12381_fr>(d, d_a, inverse, decimation, coset, st);
-  return run_fft<bls12377_fr>(d, d_a, inverse, decimation, coset, st);
+  return with_fr(d->field, [&](auto tag) { return run_fft<typename decltype(tag)::type>(d, d_a, inverse, decimation, coset, st); });
 }
 
 extern "C" int gmsm_fft_device(gmsm_fft_domain_t* d, void* d_a, size_t n, int inverse, int decimation, int coset, void* stream) {
@@ -200,9 +252,10 @@ static int fft_host(gmsm_fft_domain_t* d, uint64_t* a, size_t n, int inverse, in
   if (decimation != 0 && decimation != 1) return set_err(GMSM_EINVAL, "not implemented");  // fft.go:108
   std::lock_guard<std::mutex> lk(d->mu);
   CK(cudaSetDevice(d->device));
-  CK(cudaMemcpy(d->d_buf, a, n * 32, cudaMemcpyHostToDevice));
+  const size_t bytes = n * 8 * (size_t)d->words;
+  CK(cudaMemcpy(d->d_buf, a, bytes, cudaMemcpyHostToDevice));
   if (int rc = fft_dispatch(d, d->d_buf, inverse, decimation, coset, nullptr)) return rc;
-  CK(cudaMemcpy(a, d->d_buf, n * 32, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(a, d->d_buf, bytes, cudaMemcpyDeviceToHost));
   return GMSM_OK;
 }
 extern "C" int gmsm_fft(gmsm_fft_domain_t* d, uint64_t* a, size_t n, int decimation, int coset) { return fft_host(d, a, n, 0, decimation, coset); }
@@ -214,9 +267,10 @@ extern "C" int gmsm_fft_bit_reverse_device(gmsm_fft_domain_t* d, void* d_a, size
   std::lock_guard<std::mutex> lk(d->mu);
   CK(cudaSetDevice(d->device));
   unsigned blocks = (unsigned)std::min<uint64_t>((n + 255) / 256, GMSM_NUM_SMS * 32u);
-  if (d->field == 0) k_fft_bit_reverse<bn254_fr><<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<Fp<bn254_fr>*>(d_a), n, d->logn);
-  else if (d->field == 1) k_fft_bit_reverse<bls12381_fr><<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<Fp<bls12381_fr>*>(d_a), n, d->logn);
-  else k_fft_bit_reverse<bls12377_fr><<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<Fp<bls12377_fr>*>(d_a), n, d->logn);
-  CK(cudaGetLastError());
-  return GMSM_OK;
+  return with_fr(d->field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    k_fft_bit_reverse<P><<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<Fp<P>*>(d_a), n, d->logn);
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
 }

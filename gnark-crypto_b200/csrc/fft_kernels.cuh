@@ -5,33 +5,17 @@
 #include <cuda_runtime.h>
 
 #include "field.cuh"
+#include "vec_io.cuh"
 
 using namespace gmsm;
 
 namespace {
 
-constexpr int TILE_LOG = 10;            // stages fused in shared memory: 2^10 elements x 32 B = 32 KB per block
+// stages fused in shared memory: 2^10 elements per block, 32 KB for the 4-limb fields, 40 KB for bw6-633 and 48 KB for bw6-761
+// (48 KB is the default dynamic shared-memory limit, so no cudaFuncSetAttribute opt-in is needed).  Elements move through
+// load_vec / store_vec: 16-byte accesses for 32- and 48-byte elements, 8-byte ones for the 40-byte bw6-633 element.
+constexpr int TILE_LOG = 10;
 constexpr int TILE = 1 << TILE_LOG;
-
-template <class T>
-__device__ __forceinline__ T ldv(const T* p) {
-  T r;
-  const uint4* s = reinterpret_cast<const uint4*>(p);
-  uint32_t* w = reinterpret_cast<uint32_t*>(&r);
-#pragma unroll
-  for (int i = 0; i < (int)(sizeof(T) / 16); i++) {
-    uint4 v = s[i];
-    w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w;
-  }
-  return r;
-}
-template <class T>
-__device__ __forceinline__ void stv(T* p, const T& r) {
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(&r);
-  uint4* d = reinterpret_cast<uint4*>(p);
-#pragma unroll
-  for (int i = 0; i < (int)(sizeof(T) / 16); i++) d[i] = make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
-}
 
 // tw[t] = w^t for t < count, from pw[k] = w^(2^k)
 template <class P>
@@ -39,8 +23,8 @@ __global__ void k_fft_powers(Fp<P>* __restrict__ tw, uint64_t count, const Fp<P>
   for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < count; t += (uint64_t)gridDim.x * blockDim.x) {
     Fp<P> acc = Fp<P>::one();
     for (int k = 0; k < nbits; k++)
-      if ((t >> k) & 1ull) acc = fp_mul(acc, ldv(pw + k));
-    stv(tw + t, acc);
+      if ((t >> k) & 1ull) acc = fp_mul(acc, load_vec(pw + k));
+    store_vec(tw + t, acc);
   }
 }
 
@@ -50,10 +34,10 @@ __global__ void k_fft_dif_stage(Fp<P>* __restrict__ a, const Fp<P>* __restrict__
   for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < half_n; t += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t j = t & (h - 1), blk = t / h;
     const uint64_t i0 = blk * 2 * h + j, i1 = i0 + h;
-    Fp<P> x = ldv(a + i0), y = ldv(a + i1);
-    stv(a + i0, fp_add(x, y));
+    Fp<P> x = load_vec(a + i0), y = load_vec(a + i1);
+    store_vec(a + i0, fp_add(x, y));
     Fp<P> d = fp_sub(x, y);
-    stv(a + i1, j ? fp_mul(d, ldv(tw + j * stride)) : d);
+    store_vec(a + i1, j ? fp_mul(d, load_vec(tw + j * stride)) : d);
   }
 }
 // one DIT stage with half-size h >= TILE: (x, y) -> (x + y w, x - y w)
@@ -62,10 +46,10 @@ __global__ void k_fft_dit_stage(Fp<P>* __restrict__ a, const Fp<P>* __restrict__
   for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < half_n; t += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t j = t & (h - 1), blk = t / h;
     const uint64_t i0 = blk * 2 * h + j, i1 = i0 + h;
-    Fp<P> x = ldv(a + i0), y = ldv(a + i1);
-    if (j) y = fp_mul(y, ldv(tw + j * stride));
-    stv(a + i0, fp_add(x, y));
-    stv(a + i1, fp_sub(x, y));
+    Fp<P> x = load_vec(a + i0), y = load_vec(a + i1);
+    if (j) y = fp_mul(y, load_vec(tw + j * stride));
+    store_vec(a + i0, fp_add(x, y));
+    store_vec(a + i1, fp_sub(x, y));
   }
 }
 
@@ -77,33 +61,33 @@ __global__ void k_fft_tile(Fp<P>* __restrict__ a, const Fp<P>* __restrict__ tw, 
   Fp<P>* s = reinterpret_cast<Fp<P>*>(smem_raw);
   const uint64_t base = (uint64_t)blockIdx.x * tile;
   const uint32_t tid = threadIdx.x, half = tile >> 1;
-  stv(s + tid, ldv(a + base + tid));
-  stv(s + tid + half, ldv(a + base + tid + half));
+  store_vec(s + tid, load_vec(a + base + tid));
+  store_vec(s + tid + half, load_vec(a + base + tid + half));
   __syncthreads();
   if (IS_DIF) {
     for (uint32_t h = half; h >= 1; h >>= 1) {
       const uint32_t j = tid & (h - 1), blk = tid / h;
       const uint32_t i0 = blk * 2 * h + j, i1 = i0 + h;
-      Fp<P> x = ldv(s + i0), y = ldv(s + i1);
+      Fp<P> x = load_vec(s + i0), y = load_vec(s + i1);
       Fp<P> d = fp_sub(x, y);
-      if (j) d = fp_mul(d, ldv(tw + (uint64_t)j * ((n >> 1) / h)));
-      stv(s + i0, fp_add(x, y));
-      stv(s + i1, d);
+      if (j) d = fp_mul(d, load_vec(tw + (uint64_t)j * ((n >> 1) / h)));
+      store_vec(s + i0, fp_add(x, y));
+      store_vec(s + i1, d);
       __syncthreads();
     }
   } else {
     for (uint32_t h = 1; h <= half; h <<= 1) {
       const uint32_t j = tid & (h - 1), blk = tid / h;
       const uint32_t i0 = blk * 2 * h + j, i1 = i0 + h;
-      Fp<P> x = ldv(s + i0), y = ldv(s + i1);
-      if (j) y = fp_mul(y, ldv(tw + (uint64_t)j * ((n >> 1) / h)));
-      stv(s + i0, fp_add(x, y));
-      stv(s + i1, fp_sub(x, y));
+      Fp<P> x = load_vec(s + i0), y = load_vec(s + i1);
+      if (j) y = fp_mul(y, load_vec(tw + (uint64_t)j * ((n >> 1) / h)));
+      store_vec(s + i0, fp_add(x, y));
+      store_vec(s + i1, fp_sub(x, y));
       __syncthreads();
     }
   }
-  stv(a + base + tid, ldv(s + tid));
-  stv(a + base + tid + half, ldv(s + tid + half));
+  store_vec(a + base + tid, load_vec(s + tid));
+  store_vec(a + base + tid + half, load_vec(s + tid + half));
 }
 
 // a[i] *= scalar * u^(e(i)), e(i) = i or bitrev(i); pw[k] = u^(2^k) (nbits entries); use_shift = 0: scalar only
@@ -111,14 +95,14 @@ template <class P>
 __global__ void k_fft_scale(Fp<P>* __restrict__ a, uint64_t n, int logn, const Fp<P>* __restrict__ pw, int use_shift, int bitrev,
                             Fp<P> scalar, int use_scalar) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    Fp<P> v = ldv(a + i);
+    Fp<P> v = load_vec(a + i);
     if (use_scalar) v = fp_mul(v, scalar);
     if (use_shift) {
       const uint64_t e = bitrev ? (logn ? (__brevll(i) >> (64 - logn)) : 0ull) : i;
       for (int k = 0; k < logn; k++)
-        if ((e >> k) & 1ull) v = fp_mul(v, ldv(pw + k));
+        if ((e >> k) & 1ull) v = fp_mul(v, load_vec(pw + k));
     }
-    stv(a + i, v);
+    store_vec(a + i, v);
   }
 }
 
@@ -127,9 +111,9 @@ __global__ void k_fft_bit_reverse(Fp<P>* __restrict__ a, uint64_t n, int logn) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t r = logn ? (__brevll(i) >> (64 - logn)) : 0;
     if (r > i) {
-      Fp<P> x = ldv(a + i), y = ldv(a + r);
-      stv(a + i, y);
-      stv(a + r, x);
+      Fp<P> x = load_vec(a + i), y = load_vec(a + r);
+      store_vec(a + i, y);
+      store_vec(a + r, x);
     }
   }
 }

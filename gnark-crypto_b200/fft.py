@@ -1,8 +1,9 @@
 """Next-row N3: host-side mirror of gnark-crypto's fft package over the C ABI.
 
 Reference: ecc/bn254/fr/fft (domain.go:24-110 `Domain`, `NewDomain`; fft.go:18-190 `Decimation`, `FFT`,
-`FFTInverse`, option `OnCoset`; bitreverse.go:17-42 `BitReverse`) and ecc/bls12-381/fr/fft.
-Vectors are numpy (n, 4) uint64 arrays = []fr.Element memory (Montgomery limbs), transformed in place."""
+`FFTInverse`, option `OnCoset`; bitreverse.go:17-42 `BitReverse`) and the same package of bls12-381, bls12-377, bls24-315,
+bls24-317, bw6-633 and bw6-761.  Vectors are numpy (n, words) uint64 arrays = []fr.Element memory (Montgomery limbs;
+words = fr.Limbs: 4, 5 for bw6-633, 6 for bw6-761), transformed in place."""
 from __future__ import annotations
 
 import numpy as np
@@ -11,7 +12,7 @@ from . import _native
 from .multiexp import MultiExpError
 
 DIT, DIF = 0, 1  # fft.Decimation
-_FIELDS = {"bn254": 0, "bls12381": 1, "bls12377": 2}
+_FIELDS = {"bn254": 0, "bls12381": 1, "bls12377": 2, "bls24315": 3, "bls24317": 4, "bw6633": 5, "bw6761": 6}
 
 
 class Domain:
@@ -19,25 +20,28 @@ class Domain:
 
     def __init__(self, curve: str, m: int, shift: np.ndarray = None, device: int = 0):
         L = _native.lib()
+        if curve not in _FIELDS:
+            raise MultiExpError("unknown curve %r (FFT over Fr: %s)" % (curve, ", ".join(_FIELDS)))
+        self.words = int(L.gmsm_fft_fr_bytes(_FIELDS[curve])) // 8
         sp = None
         if shift is not None:
-            shift = np.ascontiguousarray(shift, dtype=np.uint64).reshape(4)
+            shift = np.ascontiguousarray(shift, dtype=np.uint64).reshape(self.words)
             sp = shift.ctypes.data
         self._h = L.gmsm_fft_domain_create(_FIELDS[curve], int(m), sp, device)
         if not self._h:
             raise MultiExpError(_native.last_error())
         self.device = device
         self.Cardinality = int(L.gmsm_fft_domain_cardinality(self._h))
-        c = np.zeros(20, dtype=np.uint64)
+        c = np.zeros(5 * self.words, dtype=np.uint64)
         L.gmsm_fft_domain_constants(self._h, c.ctypes.data)
-        c = c.reshape(5, 4)
+        c = c.reshape(5, self.words)
         self.Generator, self.GeneratorInv, self.CardinalityInv, self.FrMultiplicativeGen, self.FrMultiplicativeGenInv = (
             c[0].copy(), c[1].copy(), c[2].copy(), c[3].copy(), c[4].copy())
 
     def _vec(self, a):
         if not (isinstance(a, np.ndarray) and a.dtype == np.uint64 and a.flags["C_CONTIGUOUS"]):
             raise ValueError("a must be a C-contiguous numpy uint64 array (transformed in place)")
-        if a.size != 4 * self.Cardinality:
+        if a.size != self.words * self.Cardinality:
             raise MultiExpError("len(a) must equal the domain cardinality")
         return a
 

@@ -102,28 +102,82 @@ def new_srs_g1(curve: str, size: int, alpha: int, generator: np.ndarray, r_modul
     return BatchScalarMultiplication(cname, generator, encode_scalars(alphas))
 
 
-# scalar-field moduli r (fr/element.go:44-49 `q` of ecc/bn254/fr, ecc/bls12-381/fr, ecc/bls12-377/fr); fr.Element holds
-# v * 2^256 mod r (Montgomery form, 4 little-endian u64 limbs)
-FR_MODULUS = {
-    "bn254": 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001,
-    "bls12381": 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001,
-    "bls12377": 0x12AB655E9A2CA55660B44D1E5C37B00159AA76FED00000010A11800000000001,
+_TWO_BIT = dict(mask=0b11 << 6, unc=0b00 << 6, unc_inf=None, small=0b10 << 6, large=0b11 << 6, inf=0b01 << 6)
+_THREE_BIT = dict(mask=0b111 << 5, unc=0b000 << 5, unc_inf=0b010 << 5, small=0b100 << 5, large=0b101 << 5, inf=0b110 << 5)
+
+
+@dataclass(frozen=True)
+class CurveParams:
+    """What the prover and the point codec need of one pairing curve.  fr.Element / fp.Element hold v * 2^(64 * words) mod
+    the modulus (Montgomery form, little-endian u64 limbs); fr.Bytes / fp.Bytes = 8 * words (fr|fp/element.go:36-49)."""
+
+    fr_words: int           # fr.Limbs
+    fp_words: int           # fp.Limbs
+    r: int                  # scalar-field modulus
+    q: int                  # base-field modulus
+    b: int                  # y^2 = x^3 + b, as an integer mod q
+    flags: dict             # flag bits of the most significant byte of a serialised point (marshal.go:25-34)
+
+    @property
+    def fr_bytes(self) -> int:
+        return 8 * self.fr_words
+
+    @property
+    def fp_bytes(self) -> int:
+        return 8 * self.fp_words
+
+
+_Q_BW6761 = int("122E824FB83CE0AD187C94004FAFF3EB926186A81D14688528275EF8087BE41707BA638E584E91903CEBAFF25B423048689C8ED12F9FD9071DCD3DC73EBF"
+                "F2E98A116C25667A8F8160CF8AEEAF0A437E6913E6870000082F49D00000000008B", 16)
+# one entry per curve: fr/element.go and fp/element.go (q, Limbs), the curve's .go file (b), marshal.go (flags)
+CURVE_PARAMS = {
+    "bn254": CurveParams(4, 4, 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001,
+                         0x30644E72E131A029B85045B68181585D97816A916871CA8D3C208C16D87CFD47, 3, _TWO_BIT),
+    "bls12381": CurveParams(4, 6, 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001,
+                            0x1A0111EA397FE69A4B1BA7B6434BACD764774B84F38512BF6730D2A0F6B0F6241EABFFFEB153FFFFB9FEFFFFFFFFAAAB, 4, _THREE_BIT),
+    "bls12377": CurveParams(4, 6, 0x12AB655E9A2CA55660B44D1E5C37B00159AA76FED00000010A11800000000001,
+                            0x01AE3A4617C510EAC63B05C06CA1493B1A22D9F300F5138F1EF3622FBA094800170B5D44300000008508C00000000001, 1, _THREE_BIT),
+    "bls24315": CurveParams(4, 5, 0x196DEAC24A9DA12B25FC7EC9CF927A98C8C480ECE644E36419D0C5FD00C00001,
+                            0x4C23A02B586D650D3F7498BE97C5EAFDEC1D01AA27A1AE0421EE5DA52BDE5026FE802FF40300001, 1, _THREE_BIT),
+    "bls24317": CurveParams(4, 5, 0x443F917EA68DAFC2D0B097F28D83CD491CD1E79196BF0E7AF000000000000001,
+                            0x1058CA226F60892CF28FC5A0B7F9D039169A61E684C73446D6F339E43424BF7E8D512E565DAB2AAB, 4, _THREE_BIT),
+    "bw6633": CurveParams(5, 10, 0x4C23A02B586D650D3F7498BE97C5EAFDEC1D01AA27A1AE0421EE5DA52BDE5026FE802FF40300001,
+                          int("126633CC0F35F63FC1A174F01D72AB5A8FCD8C75D79D2C74E59769AD9BBDA2F8152A6C0FADEA490B8DA9F5E83F57C497E0E8850EDBDA40"
+                              "7D7B5CE7AB839C2253D369BD31147F73CD74916EA4570000D", 16), 4, _THREE_BIT),
+    "bw6761": CurveParams(6, 12, 0x01AE3A4617C510EAC63B05C06CA1493B1A22D9F300F5138F1EF3622FBA094800170B5D44300000008508C00000000001,
+                          _Q_BW6761, _Q_BW6761 - 1, _THREE_BIT),            # b = -1 (bw6-761.go)
 }
+# views of the table by field, kept for callers of the earlier per-constant dictionaries
+FR_MODULUS = {c: p.r for c, p in CURVE_PARAMS.items()}
+FP_MODULUS = {c: p.q for c, p in CURVE_PARAMS.items()}
+CURVE_B = {c: p.b for c, p in CURVE_PARAMS.items()}
+_FLAGS = {c: p.flags for c, p in CURVE_PARAMS.items()}
+
+
+def _params(curve: str) -> CurveParams:
+    return CURVE_PARAMS[curve.split("_")[0]]
+
+
+def _limbs(modulus: int) -> int:
+    """u64 limbs of an element mod `modulus` (fr.Limbs / fp.Limbs: the modulus' bit length rounded up to 64)"""
+    return (modulus.bit_length() + 63) // 64
 
 
 def _fr_decode(limbs: np.ndarray, r: int) -> list:
     """Montgomery limbs -> regular integers"""
-    rinv = pow(1 << 256, -1, r)
-    a = np.ascontiguousarray(limbs, dtype=np.uint64).reshape(-1, 4)
-    return [(int(x[0]) | int(x[1]) << 64 | int(x[2]) << 128 | int(x[3]) << 192) * rinv % r for x in a]
+    L = _limbs(r)
+    rinv = pow(1 << (64 * L), -1, r)
+    a = np.ascontiguousarray(limbs, dtype=np.uint64).reshape(-1, L)
+    return [sum(int(x[i]) << (64 * i) for i in range(L)) * rinv % r for x in a]
 
 
 def _fr_encode(vals, r: int) -> np.ndarray:
-    out = np.empty((len(vals), 4), dtype=np.uint64)
+    L = _limbs(r)
+    out = np.empty((len(vals), L), dtype=np.uint64)
     m64 = (1 << 64) - 1
     for i, v in enumerate(vals):
-        m = (v << 256) % r
-        out[i] = [m & m64, (m >> 64) & m64, (m >> 128) & m64, m >> 192]
+        m = (v << (64 * L)) % r
+        out[i] = [(m >> (64 * k)) & m64 for k in range(L)]
     return out
 
 
@@ -154,10 +208,11 @@ class OpeningProof:
 
 def Open(p: np.ndarray, point: np.ndarray, pk: ProvingKey) -> OpeningProof:
     """kzg.Open (kzg.go:180-204): ClaimedValue = p(point); H = Commit((p - p(point)) / (X - point))."""
-    p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, 4)
+    cp = _params(pk.curve)
+    p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, cp.fr_words)
     if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
         raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
-    r = FR_MODULUS[pk.curve.split("_")[0]]
+    r = cp.r
     coeffs = _fr_decode(p, r)
     a = _fr_decode(point, r)[0]
     fa = _eval(coeffs, a, r)
@@ -172,7 +227,7 @@ def Open(p: np.ndarray, point: np.ndarray, pk: ProvingKey) -> OpeningProof:
 
 def Commit(p: np.ndarray, pk: ProvingKey, *nbTasks: int) -> np.ndarray:
     """kzg.Commit (kzg.go:159-176): Digest = MultiExp(pk.G1[:len(p)], p) as an affine point"""
-    p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, 4)
+    p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, _params(pk.curve).fr_words)
     if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
         raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
     cfg = MultiExpConfig(NbTasks=nbTasks[0] if nbTasks else 0)
@@ -186,34 +241,20 @@ def Commit(p: np.ndarray, pk: ProvingKey, *nbTasks: int) -> np.ndarray:
 # ecc/bls12-381/marshal.go:830-1000).  Used for the few points a Fiat-Shamir transcript binds (G1Affine.Marshal is
 # RawBytes, marshal.go:779-782); bulk SRS decoding runs on the device (gmsm_g1_decode, csrc/decode.cu).
 # ----------------------------------------------------------------------------------------------------------------
-FP_MODULUS = {
-    "bn254": 0x30644E72E131A029B85045B68181585D97816A916871CA8D3C208C16D87CFD47,
-    "bls12381": 0x1A0111EA397FE69A4B1BA7B6434BACD764774B84F38512BF6730D2A0F6B0F6241EABFFFEB153FFFFB9FEFFFFFFFFAAAB,
-    "bls12377": 0x01AE3A4617C510EAC63B05C06CA1493B1A22D9F300F5138F1EF3622FBA094800170B5D44300000008508C00000000001,
-}
-CURVE_B = {"bn254": 3, "bls12381": 4, "bls12377": 1}     # y^2 = x^3 + b (bn254.go:12, bls12-381.go:9, bls12-377.go)
-# flag bits of the most significant byte (marshal.go:25-31 bn254: two bits; bls12-381 / bls12-377: three bits)
-_FLAGS = {
-    "bn254": dict(mask=0b11 << 6, unc=0b00 << 6, unc_inf=None, small=0b10 << 6, large=0b11 << 6, inf=0b01 << 6),
-    "bls12381": dict(mask=0b111 << 5, unc=0b000 << 5, unc_inf=0b010 << 5, small=0b100 << 5, large=0b101 << 5, inf=0b110 << 5),
-    "bls12377": dict(mask=0b111 << 5, unc=0b000 << 5, unc_inf=0b010 << 5, small=0b100 << 5, large=0b101 << 5, inf=0b110 << 5),
-}
-
-
 def _fp_words(curve: str) -> int:
-    return 4 if curve == "bn254" else 6
+    return _params(curve).fp_words
 
 
 def _fp_decode(limbs, curve: str) -> int:
     L = _fp_words(curve)
-    p = FP_MODULUS[curve]
+    p = _params(curve).q
     v = sum(int(limbs[i]) << (64 * i) for i in range(L))
     return v * pow(1 << (64 * L), -1, p) % p
 
 
 def _fp_encode(v: int, curve: str) -> np.ndarray:
     L = _fp_words(curve)
-    p = FP_MODULUS[curve]
+    p = _params(curve).q
     m = (v << (64 * L)) % p
     return np.array([(m >> (64 * i)) & (2**64 - 1) for i in range(L)], dtype=np.uint64)
 
@@ -224,7 +265,7 @@ def g1_raw_bytes(point: np.ndarray, curve: str) -> bytes:
     point = np.ascontiguousarray(point, dtype=np.uint64).reshape(2 * L)
     nb = 8 * L
     if not point.any():
-        f = _FLAGS[curve]
+        f = _params(curve).flags
         out = bytearray(2 * nb)
         out[0] = f["unc"] if f["unc_inf"] is None else f["unc_inf"]
         return bytes(out)
@@ -237,12 +278,12 @@ def g1_bytes(point: np.ndarray, curve: str) -> bytes:
     L = _fp_words(curve)
     point = np.ascontiguousarray(point, dtype=np.uint64).reshape(2 * L)
     nb = 8 * L
-    f = _FLAGS[curve]
+    f = _params(curve).flags
     if not point.any():
         out = bytearray(nb)
         out[0] = f["inf"]
         return bytes(out)
-    p = FP_MODULUS[curve]
+    p = _params(curve).q
     x, y = _fp_decode(point[:L], curve), _fp_decode(point[L:], curve)
     out = bytearray(x.to_bytes(nb, "big"))
     out[0] |= f["large"] if y > (p - 1) // 2 else f["small"]        # LexicographicallyLargest, fp/element.go:282-296
@@ -252,10 +293,11 @@ def g1_bytes(point: np.ndarray, curve: str) -> bytes:
 def g1_set_bytes(buf: bytes, curve: str):
     """G1Affine.SetBytes without the subgroup check (marshal.go:858-950) for ONE point on the host -> (point limbs, consumed).
     Raises ValueError with the reference's messages on invalid encodings."""
-    L = _fp_words(curve)
-    nb = 8 * L
-    f = _FLAGS[curve]
-    p = FP_MODULUS[curve]
+    cp = _params(curve)
+    L = cp.fp_words
+    nb = cp.fp_bytes
+    f = cp.flags
+    p = cp.q
     if len(buf) < nb:
         raise EOFError("short buffer")
     m = buf[0] & f["mask"]
@@ -283,10 +325,10 @@ def g1_set_bytes(buf: bytes, curve: str):
         return np.concatenate([_fp_encode(x, curve), _fp_encode(y, curve)]), 2 * nb
     if m not in (f["small"], f["large"]):
         raise ValueError("invalid point encoding")
-    y2 = (x * x * x + CURVE_B[curve]) % p
+    y2 = (x * x * x + cp.b) % p
     if p % 4 == 3:
         y = pow(y2, (p + 1) // 4, p)
-    else:                                   # Tonelli-Shanks (bls12-377: q = 1 mod 4, fp/element.go Sqrt)
+    else:                                   # Tonelli-Shanks (bls12-377, bls24-315, bw6-633: q = 1 mod 4, fp/element.go Sqrt)
         y = _tonelli(y2, p)
     if y is None or y * y % p != y2:
         raise ValueError("invalid compressed coordinate: square root doesn't exist")
@@ -334,8 +376,8 @@ class BatchOpeningProof:
 
 
 def _fr_marshal(limbs, r: int) -> bytes:
-    """fr.Element.Marshal (fr/element.go:868-871): 32 bytes big-endian, canonical value"""
-    return _fr_decode(np.asarray(limbs, dtype=np.uint64), r)[0].to_bytes(32, "big")
+    """fr.Element.Marshal (fr/element.go:868-871): fr.Bytes (8 * fr.Limbs) bytes big-endian, canonical value"""
+    return _fr_decode(np.asarray(limbs, dtype=np.uint64), r)[0].to_bytes(8 * _limbs(r), "big")
 
 
 def derive_gamma(point, digests, claimed_values, hf, curve: str, *data_transcript: bytes) -> int:
@@ -343,13 +385,14 @@ def derive_gamma(point, digests, claimed_values, hf, curve: str, *data_transcrip
     "gamma": H("gamma" || point || digests (RawBytes) || claimed values || extra data), read big-endian and reduced mod r
     (fr.SetBytes, fr/element.go:880-903).  `hf` is a hashlib constructor (e.g. hashlib.sha256)."""
     c = curve.split("_")[0]
-    r = FR_MODULUS[c]
+    cp = CURVE_PARAMS[c]
+    r = cp.r
     h = hf()
     h.update(b"gamma")
     h.update(_fr_marshal(point, r))
     for d in digests:
         h.update(g1_raw_bytes(d, c))
-    for v in np.ascontiguousarray(claimed_values, dtype=np.uint64).reshape(-1, 4):
+    for v in np.ascontiguousarray(claimed_values, dtype=np.uint64).reshape(-1, cp.fr_words):
         h.update(_fr_marshal(v, r))
     for b in data_transcript:
         h.update(b)
@@ -363,10 +406,11 @@ def BatchOpenSinglePoint(polynomials, digests, point: np.ndarray, hf, pk: Provin
     if len(digests) != len(polynomials):
         raise ErrInvalidNbDigests("number of digests is not the same as the number of polynomials")
     c = pk.curve.split("_")[0]
-    r = FR_MODULUS[c]
+    cp = CURVE_PARAMS[c]
+    r = cp.r
     polys = []
     for p in polynomials:
-        p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, 4)
+        p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, cp.fr_words)
         if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
             raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
         polys.append(_fr_decode(p, r))
@@ -396,11 +440,12 @@ def FoldProof(digests, proof: BatchOpeningProof, point: np.ndarray, hf, curve: s
     host, the digests with one MultiExp (`fold`, kzg.go:506-528 -- the reference calls MultiExp for it too)."""
     from .multiexp import curve_package
 
-    claimed = np.ascontiguousarray(proof.ClaimedValues, dtype=np.uint64).reshape(-1, 4)
+    c = curve.split("_")[0]
+    cp = CURVE_PARAMS[c]
+    claimed = np.ascontiguousarray(proof.ClaimedValues, dtype=np.uint64).reshape(-1, cp.fr_words)
     if len(digests) != claimed.shape[0]:
         raise ErrInvalidNbDigests("number of digests is not the same as the number of polynomials")
-    c = curve.split("_")[0]
-    r = FR_MODULUS[c]
+    r = cp.r
     gamma = derive_gamma(point, digests, claimed, hf, c, *data_transcript)
     gam = [1]
     for _ in range(1, len(digests)):
@@ -440,7 +485,7 @@ def CommitLagrange(evals, pk: ProvingKey, domain) -> np.ndarray:
 
     from .fft import DIF
 
-    ev = np.ascontiguousarray(evals, dtype=np.uint64).reshape(-1, 4)
+    ev = np.ascontiguousarray(evals, dtype=np.uint64).reshape(-1, _params(pk.curve).fr_words)
     if ev.shape[0] != domain.Cardinality:
         raise MultiExpError("len(a) must equal the domain cardinality")
     if ev.shape[0] == 0 or ev.shape[0] > pk.G1.shape[0]:

@@ -185,32 +185,42 @@ int gmsm_batch_scalar_mul(gmsm_curve_t curve, const uint64_t* base_affine, const
 /* ---- next-row N2: bulk decoding of serialised G1 points (an SRS in the standard WriteTo format -> resident bases).
  * Replaces G1Affine.SetBytes without the subgroup check -- the Decoder's NoSubgroupChecks path -- ecc/bn254/marshal.go:858-950
  * (:52-60, :952-990), ecc/bls12-381/marshal.go:886-1000: big-endian canonical X (|| Y) with the flag bits of marshal.go:25-31 in
- * the top byte; compressed points take y = (x^3 + b)^((q+1)/4) (fp.Sqrt, q = 3 mod 4) with the sign chosen by
- * LexicographicallyLargest (fp/element.go:282-296).  `bytes` is a homogeneous stream of n points: raw = 1, RawBytes
+ * the top byte (two bits for bn254, three for the others); compressed points take a square root of x^3 + b (Tonelli-Shanks, which
+ * is fp.Sqrt's (x^3 + b)^((q+1)/4) when q = 3 mod 4) with the sign chosen by LexicographicallyLargest (fp/element.go:282-296).  `bytes` is a homogeneous stream of n points: raw = 1, RawBytes
  * (2 x fp.Bytes each); raw = 0, Bytes (compressed, fp.Bytes each).  check_on_curve != 0 also verifies y^2 = x^3 + b of
  * uncompressed points (for bn254 G1, cofactor 1, that IS the reference's subgroup check).  Output: the reference's in-memory
  * G1Affine (Montgomery limbs, infinity = zeroes).  Errors are the reference's, prefixed by the index of the first bad point.
- * bn254, bls12-381: both forms; bls12-377: raw only (q = 1 mod 4). ---- */
+ * Curves: the G1 groups of bn254, bls12-381, bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761, both forms. ---- */
 int gmsm_g1_decode(gmsm_curve_t curve, const uint8_t* bytes, size_t n, int raw, int check_on_curve, uint64_t* out_points);
 /* device buffers; *d_first_error (8 bytes, device) = (index << 8 | code) of the first bad point, all-ones if none */
 int gmsm_g1_decode_device(gmsm_curve_t curve, const void* d_bytes, size_t n, int raw, int check_on_curve, void* d_points,
                           void* d_first_error, void* stream);
 
 /* ---- next-row N3: Fr FFT behind gnark-crypto's fft.Domain (ecc/bn254/fr/fft/domain.go:24-110, fft.go:31-190,
- * bitreverse.go:17-42; ecc/bls12-381/fr/fft identical).  `a` is the []fr.Element image (n x 4 u64, Montgomery),
- * transformed in place; len(a) must equal the domain cardinality.  decimation: GMSM_DIT = 0 (input bit-reversed,
+ * bitreverse.go:17-42; the fr/fft packages of bls12-381, bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761 are the same
+ * generated code with their own constants).  `a` is the []fr.Element image (n x words u64, Montgomery; words = fr.Limbs =
+ * gmsm_fft_fr_bytes / 8: 4, or 5 for bw6-633, 6 for bw6-761), transformed in place; len(a) must equal the domain cardinality.  decimation: GMSM_DIT = 0 (input bit-reversed,
  * output natural), GMSM_DIF = 1 (input natural, output bit-reversed) -- fft.Decimation, fft.go:18-23.  coset != 0
  * = fft.OnCoset().  FFTInverse includes the scaling by CardinalityInv. ---- */
 typedef struct gmsm_fft_domain gmsm_fft_domain_t;
-enum { GMSM_FR_BN254 = 0, GMSM_FR_BLS12381 = 1, GMSM_FR_BLS12377 = 2 };
+enum {
+  GMSM_FR_BN254 = 0, GMSM_FR_BLS12381 = 1, GMSM_FR_BLS12377 = 2,
+  GMSM_FR_BLS24315 = 3,  /* maxOrderRoot 22 */
+  GMSM_FR_BLS24317 = 4,  /* maxOrderRoot 60 */
+  GMSM_FR_BW6633 = 5,    /* maxOrderRoot 20: domains stop at 2^20; 5-word elements */
+  GMSM_FR_BW6761 = 6     /* maxOrderRoot 46; 6-word elements */
+};
 enum { GMSM_DIT = 0, GMSM_DIF = 1 };
-/* NewDomain(m) / NewDomain(m, WithShift(shift)): cardinality = next power of two >= m; shift = NULL selects
- * GeneratorFullMultiplicativeGroup() (5 / 7), otherwise 4 u64 Montgomery limbs */
+/* fr.Bytes of a scalar field id (32, 40 for bw6-633, 48 for bw6-761); 0 for an unknown id */
+size_t gmsm_fft_fr_bytes(int fr_field);
+/* NewDomain(m) / NewDomain(m, WithShift(shift)): cardinality = next power of two >= m (past 2^maxOrderRoot: the reference's
+ * "too big" error); shift = NULL selects GeneratorFullMultiplicativeGroup() (bn254 5, bls12-381 7, bls12-377 22, bls24-315 7,
+ * bls24-317 7, bw6-633 13, bw6-761 15), otherwise `words` u64 Montgomery limbs */
 gmsm_fft_domain_t* gmsm_fft_domain_create(int fr_field, uint64_t m, const uint64_t* shift, int device);
 void gmsm_fft_domain_free(gmsm_fft_domain_t* domain);
 uint64_t gmsm_fft_domain_cardinality(const gmsm_fft_domain_t* domain);
-/* Generator, GeneratorInv, CardinalityInv, FrMultiplicativeGen, FrMultiplicativeGenInv (5 x 4 u64, Montgomery) */
-int gmsm_fft_domain_constants(const gmsm_fft_domain_t* domain, uint64_t out[20]);
+/* Generator, GeneratorInv, CardinalityInv, FrMultiplicativeGen, FrMultiplicativeGenInv (5 x words u64, Montgomery) */
+int gmsm_fft_domain_constants(const gmsm_fft_domain_t* domain, uint64_t* out);
 int gmsm_fft(gmsm_fft_domain_t* domain, uint64_t* a, size_t n, int decimation, int coset);           /* host buffer */
 int gmsm_fft_inverse(gmsm_fft_domain_t* domain, uint64_t* a, size_t n, int decimation, int coset);   /* host buffer */
 int gmsm_fft_device(gmsm_fft_domain_t* domain, void* d_a, size_t n, int inverse, int decimation, int coset, void* stream);
