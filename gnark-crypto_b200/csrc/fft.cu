@@ -13,6 +13,11 @@
 // stage for the strided stages, one shared-memory kernel for the last (DIF) / first (DIT) TILE_LOG stages,
 // twiddles w^j (j < n/2) precomputed per domain like the reference's Domain.twiddles; coset powers are
 // computed on the fly from u^(2^k).  HBM-bound streaming work: fr.Bytes (32 / 40 / 48) per element per pass.
+//
+// Also the Fr polynomial steps of a KZG opening on device vectors (kernels and schedules in poly_kernels.cuh):
+//   eval                          ecc/bn254/kzg/kzg.go:55-63
+//   dividePolyByXminusA           ecc/bn254/kzg/kzg.go:567-582
+//   the gamma-fold of BatchOpenSinglePoint   ecc/bn254/kzg/kzg.go:302-319
 #include <cuda_runtime.h>
 
 #include <cstdio>
@@ -26,6 +31,7 @@
 using namespace gmsm;
 
 #include "fft_kernels.cuh"
+#include "poly_kernels.cuh"
 
 namespace {
 
@@ -47,6 +53,12 @@ template <class P>
 Fp<P> host_pow2k(Fp<P> x, int k) {  // x^(2^k)
   for (int i = 0; i < k; i++) x = fp_sqr(x);
   return x;
+}
+template <class P>
+bool host_is_reduced(const Fp<P>& x) {  // x < r: a valid fr.Element
+  for (int i = P::N - 1; i >= 0; i--)
+    if (x.l[i] != P::mod(i)) return x.l[i] < P::mod(i);
+  return false;
 }
 
 struct FrConsts {
@@ -270,6 +282,78 @@ extern "C" int gmsm_fft_bit_reverse_device(gmsm_fft_domain_t* d, void* d_a, size
   return with_fr(d->field, [&](auto tag) -> int {
     using P = typename decltype(tag)::type;
     k_fft_bit_reverse<P><<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<Fp<P>*>(d_a), n, d->logn);
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+// ---- Fr polynomial steps of a KZG opening (kzg.go:55-63, 567-582, 302-319) on device vectors ----
+
+extern "C" size_t gmsm_fr_poly_workspace_bytes(int fr_field, size_t n) {
+  if (!gmsm_fft_fr_bytes(fr_field) || n == 0) return 0;
+  size_t bytes = 0;
+  with_fr(fr_field, [&](auto tag) {
+    using P = typename decltype(tag)::type;
+    bytes = poly_levels(n, poly_log_l<P>() + poly_log_b<P>()).work * sizeof(Fp<P>);
+    return GMSM_OK;
+  });
+  return bytes;
+}
+
+extern "C" int gmsm_fr_poly_div_x_minus_a_device(int fr_field, const void* d_f, size_t n, const uint64_t* a, void* d_h, void* d_fa,
+                                                 void* d_work, void* stream) {
+  const size_t fb = gmsm_fft_fr_bytes(fr_field);
+  if (!fb) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0) return set_err(GMSM_EINVAL, "empty polynomial (n = 0)");
+  if (!d_f || !a || !d_fa) return set_err(GMSM_EINVAL, "null polynomial, point or value pointer");
+  if (d_h) {
+    const uintptr_t f0 = (uintptr_t)d_f, f1 = f0 + n * fb, h0 = (uintptr_t)d_h, h1 = h0 + (n - 1) * fb;
+    if (h0 < f1 && f0 < h1) return set_err(GMSM_EINVAL, "the quotient must not overlap the polynomial");
+  }
+  if (!d_work && gmsm_fr_poly_workspace_bytes(fr_field, n)) return set_err(GMSM_EINVAL, "null workspace (gmsm_fr_poly_workspace_bytes)");
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    F av;
+    memcpy(av.l, a, sizeof(F));
+    if (!host_is_reduced(av)) return set_err(GMSM_EINVAL, "the point is not a reduced fr.Element");
+    constexpr int log_l = poly_log_l<P>(), log_b = poly_log_b<P>();
+    if (((n - 1) >> (log_l + log_b)) >= 0x7fffffffull) return set_err(GMSM_EINVAL, "polynomial too large (n = %zu)", n);
+    const size_t smem = poly_smem_bytes<P>(log_l, log_b);
+    cudaStream_t st = (cudaStream_t)stream;
+    poly_div_schedule<P>(
+        reinterpret_cast<const F*>(d_f), n, av, reinterpret_cast<F*>(d_h), reinterpret_cast<F*>(d_fa), reinterpret_cast<F*>(d_work),
+        log_l, log_b,
+        [&](const F* x, uint64_t m, const PolyMults<P>& mu, F* heads, uint64_t tiles) {
+          k_poly_heads<P><<<(unsigned)tiles, 1u << log_b, smem, st>>>(x, m, mu, log_l, heads);
+        },
+        [&](const F* x, uint64_t m, const PolyMults<P>& mu, const F* carry, F* out, int shift, F* fa, uint64_t tiles) {
+          k_poly_write<P><<<(unsigned)tiles, 1u << log_b, smem, st>>>(x, m, mu, log_l, carry, out, shift, fa);
+        });
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fr_poly_fold_device(int fr_field, const void* const* d_polys, const size_t* lens, size_t k, const uint64_t* gamma,
+                                        void* d_out, size_t out_len, void* stream) {
+  if (!gmsm_fft_fr_bytes(fr_field)) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (k == 0 || out_len == 0) return set_err(GMSM_EINVAL, "nothing to fold (k = %zu, out_len = %zu)", k, out_len);
+  if (!d_polys || !lens || !gamma || !d_out) return set_err(GMSM_EINVAL, "null argument");
+  for (size_t i = 0; i < k; i++)
+    if (lens[i] && !d_polys[i]) return set_err(GMSM_EINVAL, "polynomial %zu is null", i);
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    F g;
+    memcpy(g.l, gamma, sizeof(F));
+    if (!host_is_reduced(g)) return set_err(GMSM_EINVAL, "gamma is not a reduced fr.Element");
+    std::vector<uint64_t> len(lens, lens + k);
+    const unsigned blocks = (unsigned)std::min<uint64_t>((out_len + 255) / 256, GMSM_NUM_SMS * 32u);
+    cudaStream_t st = (cudaStream_t)stream;
+    poly_fold_schedule<P>(reinterpret_cast<const F* const*>(d_polys), len.data(), k, g, [&](const PolyFoldBatch<P>& b, int accumulate) {
+      k_poly_fold<P><<<blocks, 256, 0, st>>>(reinterpret_cast<F*>(d_out), out_len, b, accumulate);
+    });
     CK(cudaGetLastError());
     return GMSM_OK;
   });

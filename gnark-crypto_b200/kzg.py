@@ -6,18 +6,24 @@
     []G1Affine memory) and the 0xdeadbeef marker that precedes it in SRS.WriteDump,
     ecc/bn254/kzg/marshal.go:70-115 -- the raw image IS the layout the device wants, so a dump streams
     straight into resident bases.
-  * kzg.Open(p, point, pk)                   ecc/bn254/kzg/kzg.go:180-204  -> eval + dividePolyByXminusA on the host
-    (Fr Horner loops, as in the reference) and one MultiExp for the quotient commitment
+  * kzg.Open(p, point, pk)                   ecc/bn254/kzg/kzg.go:180-204  -> eval + dividePolyByXminusA on the device
+    (gmsm_fr_poly_div_x_minus_a_device: one suffix scan gives f(a) and the quotient) and one MultiExp of the quotient, which
+    stays in device memory
+Polynomials are numpy (n, fr.Limbs) uint64 arrays or torch CUDA int64 tensors in the same fr.Element layout on the proving key's
+device.  Proving keys sharded over several GPUs (device = -1) open on the host (Fr loops, as in the reference).
 Only the G1 proving-key side is handled (the verifying key / pairing side is out of scope)."""
 from __future__ import annotations
 
+import ctypes
 import io
 import struct
 from dataclasses import dataclass
 
 import numpy as np
 
-from .multiexp import CURVES, BatchScalarMultiplication, MultiExpConfig, MultiExpError, ResidentBases, _words
+from . import _native
+from .fft import _FIELDS
+from .multiexp import CURVES, BatchScalarMultiplication, MultiExpConfig, MultiExpError, ResidentBases, _check, _words
 
 MARKER = 0xDEADBEEF  # utils/unsafe/dump_slice.go:78
 
@@ -69,6 +75,7 @@ class ProvingKey:
         self.curve = curve + "_g1" if not curve.endswith("_g1") else curve
         self.words = 2 * _words(CURVES[self.curve])
         self.G1 = np.ascontiguousarray(g1_points, dtype=np.uint64).reshape(-1, self.words)
+        self.device = device       # -1: sharded over GMSM_DEVICES (host scalars only)
         self._bases = ResidentBases(self.curve, self.G1, device)
         if window_tables:          # the SRS is static: trade W x the device memory for faster commitments
             self._bases.Precompute()
@@ -198,6 +205,78 @@ def _divide_by_x_minus_a(f: list, fa: int, a: int, r: int) -> list:
     return f[1:]
 
 
+def _is_device(p) -> bool:
+    """a torch tensor (device polynomial) rather than an array-like of host limbs"""
+    return hasattr(p, "data_ptr") and hasattr(p, "is_cuda")
+
+
+def _host_poly(p, words: int) -> np.ndarray:
+    if _is_device(p):
+        p = p.detach().cpu().numpy().view(np.uint64)
+    return np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, words)
+
+
+def _poly_len(p, words: int) -> int:
+    if _is_device(p):
+        if p.numel() % words:
+            raise ValueError("a device polynomial holds whole fr.Elements (%d int64 each)" % words)
+        return p.numel() // words
+    return _host_poly(p, words).shape[0]
+
+
+def _device_poly(p, words: int, device: int):
+    """p as a torch int64 tensor on cuda:device: device tensors are used in place (never modified), host arrays uploaded once"""
+    import torch
+
+    if _is_device(p):
+        if not p.is_cuda or p.device.index != device or p.dtype != torch.int64 or not p.is_contiguous():
+            raise ValueError("a device polynomial must be a contiguous torch.int64 CUDA tensor on cuda:%d" % device)
+        return p
+    h = _host_poly(p, words).view(np.int64).reshape(-1)
+    if not h.flags.writeable:           # torch.from_numpy wants a writable buffer; it is only read
+        h = h.copy()
+    return torch.from_numpy(h).to(torch.device("cuda", device))
+
+
+def _reduced(limbs, r: int) -> np.ndarray:
+    """Montgomery limbs of an fr.Element, reduced mod r (the device takes reduced elements only)"""
+    return _fr_encode([_fr_decode(limbs, r)[0]], r)[0]
+
+
+def _digest(jac: np.ndarray, w: int) -> np.ndarray:
+    return jac[:w].copy() if jac[w:].any() else np.zeros(w, dtype=np.uint64)
+
+
+class _DevicePoly:
+    """gmsm_fr_poly_* of one proving key's curve on its device, ordered on the device's current torch stream"""
+
+    def __init__(self, pk: ProvingKey, max_len: int):
+        import torch
+
+        self.torch = torch
+        self.field = _FIELDS[pk.curve.split("_")[0]]
+        self.words = _params(pk.curve).fr_words
+        self.dev = torch.device("cuda", pk.device)
+        self.stream = torch.cuda.current_stream(self.dev).cuda_stream
+        ws = int(_native.lib().gmsm_fr_poly_workspace_bytes(self.field, max_len))
+        self.work = torch.empty(ws // 8, dtype=torch.int64, device=self.dev) if ws else None
+
+    def empty(self, n: int):
+        return self.torch.empty(n * self.words, dtype=self.torch.int64, device=self.dev)
+
+    def div(self, d_f, n: int, a: np.ndarray, d_h, d_fa):
+        """d_fa = f(a); d_h = (f - f(a)) / (X - a) unless None"""
+        _check(_native.lib().gmsm_fr_poly_div_x_minus_a_device(
+            self.field, d_f.data_ptr(), n, a.ctypes.data, None if d_h is None else d_h.data_ptr(), d_fa.data_ptr(),
+            None if self.work is None else self.work.data_ptr(), self.stream))
+
+    def fold(self, d_polys, lens, gamma: np.ndarray, d_out, out_len: int):
+        ptrs = (ctypes.c_void_p * len(d_polys))(*[d.data_ptr() for d in d_polys])
+        ln = np.array(lens, dtype=np.uint64)
+        _check(_native.lib().gmsm_fr_poly_fold_device(self.field, ptrs, ln.ctypes.data, len(d_polys), gamma.ctypes.data, d_out.data_ptr(),
+                                                       out_len, self.stream))
+
+
 @dataclass
 class OpeningProof:
     """kzg.OpeningProof{H G1Affine, ClaimedValue fr.Element} (kzg.go:43-51), both in Go memory layout"""
@@ -206,13 +285,30 @@ class OpeningProof:
     ClaimedValue: np.ndarray
 
 
-def Open(p: np.ndarray, point: np.ndarray, pk: ProvingKey) -> OpeningProof:
-    """kzg.Open (kzg.go:180-204): ClaimedValue = p(point); H = Commit((p - p(point)) / (X - point))."""
+def Open(p, point: np.ndarray, pk: ProvingKey) -> OpeningProof:
+    """kzg.Open (kzg.go:180-204): ClaimedValue = p(point); H = Commit((p - p(point)) / (X - point)).  On a single-device proving key
+    the value and the quotient come from one scan on the device and the quotient feeds the MultiExp there; only f(a) and H come
+    back."""
     cp = _params(pk.curve)
-    p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, cp.fr_words)
+    r = cp.r
+    if pk.device >= 0:
+        n = _poly_len(p, cp.fr_words)
+        # n == 1: Commit of the empty quotient errors in the reference (kzg.go:160-162): a constant polynomial cannot be opened
+        if n <= 1 or n > pk.G1.shape[0]:
+            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        import torch
+
+        with torch.cuda.device(pk.device):
+            dp = _DevicePoly(pk, n)
+            d_f = _device_poly(p, cp.fr_words, pk.device)
+            d_h, d_fa = dp.empty(n - 1), dp.empty(1)
+            dp.div(d_f, n, _reduced(point, r), d_h, d_fa)
+            jac = pk._bases.MultiExpDevice(d_h, n - 1, stream=dp.stream)
+            fa = d_fa.cpu().numpy().view(np.uint64)
+        return OpeningProof(H=_digest(jac, pk.words), ClaimedValue=fa.copy())
+    p = _host_poly(p, cp.fr_words)
     if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
         raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
-    r = cp.r
     coeffs = _fr_decode(p, r)
     a = _fr_decode(point, r)[0]
     fa = _eval(coeffs, a, r)
@@ -225,15 +321,25 @@ def Open(p: np.ndarray, point: np.ndarray, pk: ProvingKey) -> OpeningProof:
     return OpeningProof(H=H.reshape(w), ClaimedValue=_fr_encode([fa], r)[0])
 
 
-def Commit(p: np.ndarray, pk: ProvingKey, *nbTasks: int) -> np.ndarray:
-    """kzg.Commit (kzg.go:159-176): Digest = MultiExp(pk.G1[:len(p)], p) as an affine point"""
-    p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, _params(pk.curve).fr_words)
+def Commit(p, pk: ProvingKey, *nbTasks: int) -> np.ndarray:
+    """kzg.Commit (kzg.go:159-176): Digest = MultiExp(pk.G1[:len(p)], p) as an affine point.  A device polynomial (torch tensor)
+    goes straight to the MultiExp on a single-device proving key."""
+    words = _params(pk.curve).fr_words
+    cfg = MultiExpConfig(NbTasks=nbTasks[0] if nbTasks else 0)
+    if _is_device(p) and pk.device >= 0:
+        n = _poly_len(p, words)
+        if n == 0 or n > pk.G1.shape[0]:
+            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        import torch
+
+        with torch.cuda.device(pk.device):
+            d = _device_poly(p, words, pk.device)
+            jac = pk._bases.MultiExpDevice(d, n, cfg, stream=torch.cuda.current_stream(d.device).cuda_stream)
+        return _digest(jac, pk.words)
+    p = _host_poly(p, words)
     if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
         raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
-    cfg = MultiExpConfig(NbTasks=nbTasks[0] if nbTasks else 0)
-    jac = pk._bases.MultiExp(p, cfg)
-    w = pk.words
-    return jac[:w].copy() if jac[w:].any() else np.zeros(w, dtype=np.uint64)
+    return _digest(pk._bases.MultiExp(p, cfg), pk.words)
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -401,16 +507,19 @@ def derive_gamma(point, digests, claimed_values, hf, curve: str, *data_transcrip
 
 def BatchOpenSinglePoint(polynomials, digests, point: np.ndarray, hf, pk: ProvingKey, *data_transcript: bytes) -> BatchOpeningProof:
     """kzg.BatchOpenSinglePoint (kzg.go:246-331): ClaimedValues[i] = f_i(point); gamma by Fiat-Shamir; the folded polynomial
-    sum_i gamma^i f_i is divided by (X - point) on the host (Fr loops, as in the reference) and committed with ONE MultiExp
-    over the resident bases."""
+    sum_i gamma^i f_i is divided by (X - point) and committed with ONE MultiExp over the resident bases.  On a single-device
+    proving key the evaluations, the fold and the division run on the device: the claimed values come back in one copy for
+    the transcript, the folded polynomial and its quotient never leave the device."""
     if len(digests) != len(polynomials):
         raise ErrInvalidNbDigests("number of digests is not the same as the number of polynomials")
     c = pk.curve.split("_")[0]
     cp = CURVE_PARAMS[c]
     r = cp.r
+    if pk.device >= 0:
+        return _batch_open_device(polynomials, digests, point, hf, pk, *data_transcript)
     polys = []
     for p in polynomials:
-        p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, cp.fr_words)
+        p = _host_poly(p, cp.fr_words)
         if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
             raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
         polys.append(_fr_decode(p, r))
@@ -433,6 +542,38 @@ def BatchOpenSinglePoint(polynomials, digests, point: np.ndarray, hf, pk: Provin
         raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
     H = Commit(_fr_encode(h, r), pk)
     return BatchOpeningProof(H=H.reshape(pk.words), ClaimedValues=claimed_limbs)
+
+
+def _batch_open_device(polynomials, digests, point, hf, pk: ProvingKey, *data_transcript: bytes) -> BatchOpeningProof:
+    import torch
+
+    c = pk.curve.split("_")[0]
+    cp = CURVE_PARAMS[c]
+    r, w = cp.r, cp.fr_words
+    lens = []
+    for p in polynomials:
+        n = _poly_len(p, w)
+        if n == 0 or n > pk.G1.shape[0]:
+            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        lens.append(n)
+    largest = max(lens)
+    a = _reduced(point, r)
+    with torch.cuda.device(pk.device):
+        dp = _DevicePoly(pk, largest)
+        d_polys = [_device_poly(p, w, pk.device) for p in polynomials]
+        d_claimed = dp.empty(len(lens))
+        for i, (d_f, n) in enumerate(zip(d_polys, lens)):
+            dp.div(d_f, n, a, None, d_claimed[i * w:(i + 1) * w])
+        claimed_limbs = d_claimed.cpu().numpy().view(np.uint64).reshape(-1, w).copy()
+        gamma = derive_gamma(point, digests, claimed_limbs, hf, c, *data_transcript)
+        if largest == 1:        # the folded quotient is empty: Commit errors in the reference
+            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        d_fold = dp.empty(largest)
+        dp.fold(d_polys, lens, _fr_encode([gamma], r)[0], d_fold, largest)
+        d_h, d_fa = dp.empty(largest - 1), dp.empty(1)
+        dp.div(d_fold, largest, a, d_h, d_fa)
+        jac = pk._bases.MultiExpDevice(d_h, largest - 1, stream=dp.stream)
+    return BatchOpeningProof(H=_digest(jac, pk.words), ClaimedValues=claimed_limbs)
 
 
 def FoldProof(digests, proof: BatchOpeningProof, point: np.ndarray, hf, curve: str, *data_transcript: bytes):

@@ -226,6 +226,22 @@ int gmsm_fft_inverse(gmsm_fft_domain_t* domain, uint64_t* a, size_t n, int decim
 int gmsm_fft_device(gmsm_fft_domain_t* domain, void* d_a, size_t n, int inverse, int decimation, int coset, void* stream);
 int gmsm_fft_bit_reverse_device(gmsm_fft_domain_t* domain, void* d_a, size_t n, void* stream);        /* fft.BitReverse */
 
+/* ---- the Fr polynomial steps of kzg.Open / kzg.BatchOpenSinglePoint on device vectors: eval (ecc/bn254/kzg/kzg.go:55-63),
+ * dividePolyByXminusA (:567-582) and the gamma-fold (:302-319); the same for the other six scalar fields.  Vectors are device
+ * []fr.Element images (n x fr.Limbs u64, Montgomery, reduced) on the current device; the work is ordered on `stream` (a
+ * cudaStream_t, NULL = default stream) and nothing is allocated inside a call.  Host scalars (a, gamma) are fr.Limbs u64
+ * Montgomery limbs and must be reduced.  Results are the reference's limbs. ---- */
+/* bytes of device workspace gmsm_fr_poly_div_x_minus_a_device needs for n coefficients (0: none; 0 for an unknown field) */
+size_t gmsm_fr_poly_workspace_bytes(int fr_field, size_t n);
+/* *d_fa = f(a) (one element) and, when d_h != NULL, d_h[0, n-1) = (f - f(a)) / (X - a); d_h must not overlap d_f, which is
+ * left unchanged (the reference divides a copy).  d_h = NULL: evaluation only.  n = 0 is GMSM_EINVAL. */
+int gmsm_fr_poly_div_x_minus_a_device(int fr_field, const void* d_f, size_t n, const uint64_t* a, void* d_h, void* d_fa,
+                                      void* d_work, void* stream);
+/* d_out[j] = sum_i gamma^i f_i[j] for j < out_len, f_i zero past lens[i] (gamma^0 = 1); d_polys: host array of k device
+ * pointers, each input read once */
+int gmsm_fr_poly_fold_device(int fr_field, const void* const* d_polys, const size_t* lens, size_t k, const uint64_t* gamma,
+                             void* d_out, size_t out_len, void* stream);
+
 /* ---- 5. test hooks: element-wise device functions, used by tests/ to check the sm_90a field and
  * point arithmetic against the oracle.  a, b, out are HOST arrays of n elements each. ---- */
 enum {
