@@ -139,7 +139,14 @@ struct GroupVTable {
   int (*digits_dump)(const void* d_scalars, size_t n, int c, int nwin, uint32_t* dout);
   int (*batch_scalar_mul)(const void* d_table, const void* d_scalars, size_t n, int c, int nwin, void* d_out, cudaStream_t);
   int (*table_level)(const void* d_in, size_t n, int c, void* d_out, cudaStream_t);   // out[i] = 2^c * in[i]
+  // kzg.ToLagrangeG1 (lagrange_kernels.cuh) on n = 2^k >= 2 affine points: w_inv = fr.Generator(n)^-1 and n_inv = 1/n as
+  // Montgomery fr limbs, d_work holds n extended-Jacobian points.  Null except for the G1 groups of the pairing curves.
+  int (*to_lagrange)(const void* d_points, size_t n, const uint64_t* w_inv, const uint64_t* n_inv, void* d_out, void* d_work,
+                     cudaStream_t);
 };
+// fr.Generator(n)^-1 and 1/n of the scalar field fr_field (GMSM_FR_*) as Montgomery u64 limbs, n a power of two (fft.cu); the
+// error of fr.Generator past maxOrderRoot
+int fr_domain_inverses(int fr_field, uint64_t n, uint64_t* w_inv, uint64_t* n_inv);
 extern const GroupVTable vt_bn254_g1, vt_bn254_g2, vt_bls12381_g1, vt_bls12381_g2, vt_bls12377_g1, vt_bls12377_g2, vt_secp256k1_g1,
     vt_bw6761_g1, vt_bw6761_g2, vt_bls24315_g1, vt_bls24317_g1, vt_bw6633_g1, vt_bw6633_g2;
 

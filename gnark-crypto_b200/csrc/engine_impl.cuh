@@ -1,8 +1,11 @@
 // Template orchestration of the kernels for one (curve, group); included by inst_*.cu.
 #pragma once
+#include <cstring>
+
 #include "engine.h"
 #include "kernels.cuh"
 #include "affine_kernels.cuh"
+#include "lagrange_kernels.cuh"
 
 namespace gmsm {
 
@@ -347,8 +350,41 @@ static int run_table_level(const void* d_in, size_t n, int c, void* d_out, cudaS
   return GMSM_OK;
 }
 
+// kzg.ToLagrangeG1 (lagrange_kernels.cuh): logn stage launches, then the finish launch, all on st
+template <class G>
+static int run_to_lagrange(const void* d_points, size_t n, const uint64_t* w_inv, const uint64_t* n_inv, void* d_out, void* d_work,
+                           cudaStream_t st) {
+  using F = typename G::F;
+  using Fr = typename G::Fr;
+  int logn = 0;
+  while (((size_t)1 << logn) < n) logn++;
+  Fr wi, ni;
+  memcpy(wi.l, w_inv, sizeof(Fr));
+  memcpy(ni.l, n_inv, sizeof(Fr));
+  const LagPowers<G> pw = lag_powers<G>(wi, logn);
+  const auto* in = reinterpret_cast<const Affine<F>*>(d_points);
+  auto* ws = reinterpret_cast<XYZZ<F>*>(d_work);
+  lagrange_schedule(
+      n, logn,
+      [&](int s, uint64_t threads) {
+        if (s == 0)
+          k_lag_stage<G, true><<<nblk(threads, 128), 128, 0, st>>>(in, ws, (uint32_t)threads, logn, s, pw);
+        else
+          k_lag_stage<G, false><<<nblk(threads, 128), 128, 0, st>>>(in, ws, (uint32_t)threads, logn, s, pw);
+      },
+      [&](uint64_t threads) {
+        k_lag_finish<G><<<nblk(threads, 128), 128, 0, st>>>(ws, (uint32_t)n, logn, ni, reinterpret_cast<Affine<F>*>(d_out));
+      });
+  LAUNCH_CHECK();
+  return GMSM_OK;
+}
+
 #define GMSM_INSTANTIATE(G, NAME)                                                                  \
   const GroupVTable NAME = {&run_window_sums<G>, &run_accumulate<G>, &run_bucket_reduce<G>, &run_finalize<G>, &run_generate<G>, &test_op_sizes<G>, \
                             &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>};
+// the G1 groups of the seven pairing curves: also kzg.ToLagrangeG1
+#define GMSM_INSTANTIATE_PAIRING_G1(G, NAME)                                                       \
+  const GroupVTable NAME = {&run_window_sums<G>, &run_accumulate<G>, &run_bucket_reduce<G>, &run_finalize<G>, &run_generate<G>, &test_op_sizes<G>, \
+                            &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>, &run_to_lagrange<G>};
 
 }  // namespace gmsm

@@ -192,6 +192,24 @@ static int run_fft(gmsm_fft_domain* d, void* d_a, int inverse, int decimation, i
   return GMSM_OK;
 }
 
+// the domain inverses of kzg.ToLagrangeG1 (computeTwiddlesInv, ecc/bn254/kzg/utils.go:66-93): the same root as a domain of n
+int gmsm::fr_domain_inverses(int fr_field, uint64_t n, uint64_t* w_inv, uint64_t* n_inv) {
+  const FrConsts* fcp = fr_consts(fr_field);
+  if (!fcp) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  int logn = 0;
+  while (((uint64_t)1 << logn) < n) logn++;
+  if (logn > fcp->max_order)
+    return set_err(GMSM_EINVAL, "m (%llu) is too big: the required root of unity does not exist", (unsigned long long)n);  // generator.go:29
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    const Fp<P> wi = fp_inv(host_pow2k(host_from_decimal<P>(fcp->root), fcp->max_order - logn));
+    const Fp<P> ni = fp_inv(host_from_u64<P>(n));
+    memcpy(w_inv, wi.l, sizeof(Fp<P>));
+    memcpy(n_inv, ni.l, sizeof(Fp<P>));
+    return GMSM_OK;
+  });
+}
+
 extern "C" gmsm_fft_domain_t* gmsm_fft_domain_create(int fr_field, uint64_t m, const uint64_t* shift, int device) {
   const FrConsts* fcp = fr_consts(fr_field);
   if (!fcp) { set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field); return nullptr; }

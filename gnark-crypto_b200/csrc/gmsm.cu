@@ -1332,6 +1332,78 @@ extern "C" int gmsm_batch_scalar_mul(gmsm_curve_t curve, const uint64_t* base_af
 }
 
 // ------------------------------------------------------------------------------------------
+// kzg.ToLagrangeG1 (ecc/<curve>/kzg/utils.go:25-64): inverse FFT over G1 points (lagrange_kernels.cuh)
+// ------------------------------------------------------------------------------------------
+static int lagrange_fr_field(int curve) {   // the scalar field of a pairing curve's G1 group, -1 for the other groups
+  switch (curve) {
+    case GMSM_BN254_G1: return GMSM_FR_BN254;
+    case GMSM_BLS12381_G1: return GMSM_FR_BLS12381;
+    case GMSM_BLS12377_G1: return GMSM_FR_BLS12377;
+    case GMSM_BLS24315_G1: return GMSM_FR_BLS24315;
+    case GMSM_BLS24317_G1: return GMSM_FR_BLS24317;
+    case GMSM_BW6633_G1: return GMSM_FR_BW6633;
+    case GMSM_BW6761_G1: return GMSM_FR_BW6761;
+  }
+  return -1;
+}
+
+extern "C" size_t gmsm_g1_to_lagrange_workspace_bytes(gmsm_curve_t curve, size_t n) {
+  return lagrange_fr_field(curve) < 0 ? 0 : n * gmsm_xyzz_bytes(curve);
+}
+
+// the argument checks of both entry points, before any device work: curve, then the reference's order (power of two, root)
+static int to_lagrange_args(int curve, size_t n, uint64_t* w_inv, uint64_t* n_inv) {
+  CurveInfo ci;
+  if (!curve_info(curve, &ci)) return set_err(GMSM_EINVAL, "unknown curve id %d", curve);
+  const int field = lagrange_fr_field(curve);
+  if (field < 0 || !vtable(curve)->to_lagrange)
+    return set_err(GMSM_EINVAL, "ToLagrangeG1 is provided for the G1 groups of the pairing curves only (curve id %d)", curve);
+  if (n == 0 || (n & (n - 1)) != 0) return set_err(GMSM_EINVAL, "len(coeffs) must be a power of 2");   // utils.go:26-28
+  if (int rc = fr_domain_inverses(field, n, w_inv, n_inv)) return rc;                                  // utils.go:33-36
+  if (n > ((size_t)1 << LAG_MAX_LOG)) return set_err(GMSM_EINVAL, "len(coeffs) = %zu exceeds 2^%d", n, LAG_MAX_LOG);
+  return GMSM_OK;
+}
+
+extern "C" int gmsm_g1_to_lagrange_device(gmsm_curve_t curve, const void* d_points, size_t n, void* d_out, void* d_work, void* stream) {
+  uint64_t w_inv[6], n_inv[6];
+  if (int rc = to_lagrange_args(curve, n, w_inv, n_inv)) return rc;
+  if (!d_points || !d_out) return set_err(GMSM_EINVAL, "null point array");
+  if (n > 1 && !d_work) return set_err(GMSM_EINVAL, "null workspace (gmsm_g1_to_lagrange_workspace_bytes)");
+  if (int rc = set_device_of(d_out)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n == 1) {   // [1]P = P
+    if (d_out != d_points) CK(cudaMemcpyAsync(d_out, d_points, gmsm_affine_bytes(curve), cudaMemcpyDeviceToDevice, st));
+    return GMSM_OK;
+  }
+  return vtable(curve)->to_lagrange(d_points, n, w_inv, n_inv, d_out, d_work, st);
+}
+
+extern "C" int gmsm_g1_to_lagrange(gmsm_curve_t curve, const uint64_t* points, size_t n, int device, uint64_t* out) {
+  uint64_t w_inv[6], n_inv[6];
+  if (int rc = to_lagrange_args(curve, n, w_inv, n_inv)) return rc;
+  if (!points || !out) return set_err(GMSM_EINVAL, "null point array");
+  if (int rc = check_device(device)) return rc;
+  CK(cudaSetDevice(device));
+  const size_t bytes = n * gmsm_affine_bytes(curve);
+  void *d_pts = nullptr, *d_work = nullptr;
+  cudaStream_t st = nullptr;
+  auto cleanup = [&]() { cudaFree(d_pts); cudaFree(d_work); if (st) cudaStreamDestroy(st); };
+  if (cudaMalloc(&d_pts, bytes) != cudaSuccess || cudaMalloc(&d_work, std::max<size_t>(gmsm_g1_to_lagrange_workspace_bytes(curve, n), 16)) != cudaSuccess ||
+      cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) {
+    cleanup();
+    return set_err(GMSM_ENOMEM, "gmsm_g1_to_lagrange: device allocation failed (n = %zu)", n);
+  }
+  int rc = GMSM_OK;
+  cudaError_t ce = cudaMemcpyAsync(d_pts, points, bytes, cudaMemcpyHostToDevice, st);
+  if (ce == cudaSuccess) rc = gmsm_g1_to_lagrange_device(curve, d_pts, n, d_pts, d_work, st);
+  if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpyAsync(out, d_pts, bytes, cudaMemcpyDeviceToHost, st);
+  if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaStreamSynchronize(st);
+  if (ce != cudaSuccess) rc = set_err(GMSM_ECUDA, "gmsm_g1_to_lagrange: %s", cudaGetErrorString(ce));
+  cleanup();
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------
 // test hooks
 // ------------------------------------------------------------------------------------------
 namespace {

@@ -55,6 +55,9 @@ static constexpr int SCAN_THREADS = 256;
 static constexpr int SCAN_ITEMS = 8;                              // per thread
 static constexpr int SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;       // per block
 
+// kzg.ToLagrangeG1 (lagrange_kernels.cuh) takes n <= 2^LAG_MAX_LOG points: butterfly and output indices fit in 32 bits
+static constexpr int LAG_MAX_LOG = 31;
+
 // ---- window plan (computeNbChunks / lastC, ecc/bn254/multiexp.go:681-693) ----
 struct WindowPlan {
   int c;          // window width in bits

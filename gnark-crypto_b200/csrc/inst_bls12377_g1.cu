@@ -14,5 +14,5 @@
 #endif
 #include "engine_impl.cuh"
 namespace gmsm {
-GMSM_INSTANTIATE(bls12377_g1, vt_bls12377_g1)
+GMSM_INSTANTIATE_PAIRING_G1(bls12377_g1, vt_bls12377_g1)
 }

@@ -14,5 +14,5 @@
 #endif
 #include "engine_impl.cuh"
 namespace gmsm {
-GMSM_INSTANTIATE(bls24317_g1, vt_bls24317_g1)
+GMSM_INSTANTIATE_PAIRING_G1(bls24317_g1, vt_bls24317_g1)
 }

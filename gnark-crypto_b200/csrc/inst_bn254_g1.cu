@@ -17,5 +17,5 @@
 #endif
 #include "engine_impl.cuh"
 namespace gmsm {
-GMSM_INSTANTIATE(bn254_g1, vt_bn254_g1)
+GMSM_INSTANTIATE_PAIRING_G1(bn254_g1, vt_bn254_g1)
 }

@@ -10,5 +10,5 @@
 #endif
 #include "engine_impl.cuh"
 namespace gmsm {
-GMSM_INSTANTIATE(bw6633_g1, vt_bw6633_g1)
+GMSM_INSTANTIATE_PAIRING_G1(bw6633_g1, vt_bw6633_g1)
 }

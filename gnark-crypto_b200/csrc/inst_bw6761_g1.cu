@@ -12,5 +12,5 @@
 #endif
 #include "engine_impl.cuh"
 namespace gmsm {
-GMSM_INSTANTIATE(bw6761_g1, vt_bw6761_g1)
+GMSM_INSTANTIATE_PAIRING_G1(bw6761_g1, vt_bw6761_g1)
 }

@@ -9,6 +9,8 @@
   * kzg.Open(p, point, pk)                   ecc/bn254/kzg/kzg.go:180-204  -> eval + dividePolyByXminusA on the device
     (gmsm_fr_poly_div_x_minus_a_device: one suffix scan gives f(a) and the quotient) and one MultiExp of the quotient, which
     stays in device memory
+  * kzg.ToLagrangeG1(coeffs)                 ecc/bn254/kzg/utils.go:25-64 -> inverse FFT over G1 points on the device
+    (gmsm_g1_to_lagrange, csrc/lagrange_kernels.cuh)
 Polynomials are numpy (n, fr.Limbs) uint64 arrays or torch CUDA int64 tensors in the same fr.Element layout on the proving key's
 device.  Proving keys sharded over several GPUs (device = -1) open on the host (Fr loops, as in the reference).
 Only the G1 proving-key side is handled (the verifying key / pairing side is out of scope)."""
@@ -614,6 +616,38 @@ def decode_g1_points(curve: str, data: bytes, n: int, raw: bool = False, check_o
     rc = _native.lib().gmsm_g1_decode(CURVES[cname], buf.ctypes.data, n, 1 if raw else 0, 1 if check_on_curve else 0, out.ctypes.data)
     if rc != 0:
         raise MultiExpError(_native.last_error())
+    return out
+
+
+def ToLagrangeG1(coeffs, curve: str, device: int = 0):
+    """kzg.ToLagrangeG1 (utils.go:25-64): the Lagrange form [L_i(tau)]G of a canonical SRS [tau^i]G, by an inverse FFT over G1
+    points on the GPU (gmsm_g1_to_lagrange, csrc/lagrange_kernels.cuh).  `coeffs`: (n, 2 * fp.Limbs) uint64 array of G1Affine in Go
+    memory layout, n a power of two; returns a new array in the affine normal form.  A torch CUDA int64 tensor in the same layout is
+    transformed on its own device, on the current stream, into a new tensor (the input is left unmodified, nothing visits the
+    host).  ProvingKey(curve, ToLagrangeG1(srs, curve)) is the Lagrange-form key: Commit of evaluations on the domain of size n
+    with it equals CommitLagrange with the canonical key.  Errors are MultiExpError with the reference's texts."""
+    cname = curve if curve.endswith(("_g1", "_g2")) else curve + "_g1"
+    if cname not in CURVES:
+        raise MultiExpError("unknown curve %r" % curve)
+    cid = CURVES[cname]
+    words = 2 * _words(cid)
+    L = _native.lib()
+    if _is_device(coeffs):
+        import torch
+
+        if not coeffs.is_cuda or coeffs.dtype != torch.int64 or not coeffs.is_contiguous() or coeffs.numel() % words:
+            raise ValueError("device points must be a contiguous torch.int64 CUDA tensor of (n, %d) words" % words)
+        n = coeffs.numel() // words
+        out = torch.empty_like(coeffs)
+        with torch.cuda.device(coeffs.device):
+            ws = int(L.gmsm_g1_to_lagrange_workspace_bytes(cid, n))
+            work = torch.empty(max(ws // 8, 1), dtype=torch.int64, device=coeffs.device)
+            st = torch.cuda.current_stream(coeffs.device).cuda_stream
+            _check(L.gmsm_g1_to_lagrange_device(cid, coeffs.data_ptr(), n, out.data_ptr(), work.data_ptr(), st))
+        return out
+    pts = np.ascontiguousarray(coeffs, dtype=np.uint64).reshape(-1, words)
+    out = np.empty_like(pts)
+    _check(L.gmsm_g1_to_lagrange(cid, pts.ctypes.data, pts.shape[0], device, out.ctypes.data))
     return out
 
 

@@ -242,6 +242,21 @@ int gmsm_fr_poly_div_x_minus_a_device(int fr_field, const void* d_f, size_t n, c
 int gmsm_fr_poly_fold_device(int fr_field, const void* const* d_polys, const size_t* lens, size_t k, const uint64_t* gamma,
                              void* d_out, size_t out_len, void* stream);
 
+/* ---- kzg.ToLagrangeG1 (ecc/bn254/kzg/utils.go:25-64; the same for the other pairing curves): the canonical SRS [tau^i]G in,
+ * its Lagrange form [L_i(tau)]G out, by an inverse FFT over G1 points on the device.  Curves: the G1 groups of bn254, bls12-381,
+ * bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761 (others: GMSM_EINVAL).  Points are the reference's in-memory G1Affine
+ * (Montgomery limbs, infinity = zeroes), output in the affine normal form of BatchJacobianToAffineG1.  Errors, checked before
+ * any device work: "len(coeffs) must be a power of 2" (n = 0 included) and fr.Generator's "m (<n>) is too big: the required
+ * root of unity does not exist" (bls24-315 past 2^22, bw6-633 past 2^20); n is at most 2^31. ---- */
+/* bytes of device workspace for n points (n extended-Jacobian points); 0 for unsupported curves */
+size_t gmsm_g1_to_lagrange_workspace_bytes(gmsm_curve_t curve, size_t n);
+/* host buffers; the input is left unmodified, out may equal points */
+int gmsm_g1_to_lagrange(gmsm_curve_t curve, const uint64_t* points, size_t n, int device, uint64_t* out);
+/* device buffers on the same device, ordered on `stream` (a cudaStream_t, NULL = default stream); nothing is allocated inside
+ * the call.  d_points is left unmodified unless d_out == d_points (allowed: in place); d_work holds
+ * gmsm_g1_to_lagrange_workspace_bytes(curve, n) bytes (unused for n = 1). */
+int gmsm_g1_to_lagrange_device(gmsm_curve_t curve, const void* d_points, size_t n, void* d_out, void* d_work, void* stream);
+
 /* ---- 5. test hooks: element-wise device functions, used by tests/ to check the sm_90a field and
  * point arithmetic against the oracle.  a, b, out are HOST arrays of n elements each. ---- */
 enum {

@@ -8,6 +8,7 @@
 //        ecc/bn254/multiexp.go:32 (G1Affine :20, G2Jac :357, G2Affine :345), ecc/bls12-381/multiexp.go:20-355
 //   ecc.MultiExpConfig{NbTasks int}                                      ecc/ecc.go:107-110
 //   errors: "len(points) != len(scalars)" (multiexp.go:61-64), "invalid config: config.NbTasks > 1024" (:69-71)
+//   kzg.ToLagrangeG1(coeffs []G1Affine) ([]G1Affine, error)              ecc/<curve>/kzg/utils.go:25-64 (pairing curves)
 //
 // Types are the reference's memory images: Element<L> = [L]uint64 little-endian Montgomery limbs.
 #pragma once
@@ -35,6 +36,7 @@ using Element = std::array<uint64_t, L>;
 // EXT = 1: coordinates in Fp, 2: in Fp2 (E2{A0,A1}); LR = fr.Limbs (4; 5 for bw6-633, 6 for bw6-761)
 template <gmsm_curve_t CURVE, int L, int EXT, int LR = 4>
 struct Group {
+  static constexpr gmsm_curve_t curve = CURVE;
   using Coord = std::array<uint64_t, L * EXT>;
   using Scalar = Element<LR>;  // fr.Element
 
@@ -116,6 +118,21 @@ struct Group {
   }
 };
 
+// kzg.ToLagrangeG1 (ecc/<curve>/kzg/utils.go:25-64): the Lagrange form of a canonical SRS, len(coeffs) a power of two; the
+// input is left unmodified.  Wrapped below as <curve>::ToLagrangeG1 for the seven pairing curves.
+template <class G1>
+std::vector<typename G1::Affine> to_lagrange_g1(const std::vector<typename G1::Affine>& coeffs, int device) {
+  std::vector<typename G1::Affine> out(coeffs.size());
+  int rc = gmsm_g1_to_lagrange(G1::curve, coeffs.empty() ? nullptr : coeffs[0].X.data(), coeffs.size(), device,
+                               out.empty() ? nullptr : out[0].X.data());
+  if (rc != GMSM_OK) throw Error(gmsm_last_error());
+  return out;
+}
+#define GMSM_HOST_TO_LAGRANGE                                                                                          \
+  inline std::vector<G1Affine> ToLagrangeG1(const std::vector<G1Affine>& coeffs, int device = 0) {                  \
+    return to_lagrange_g1<G1>(coeffs, device);                                                                       \
+  }
+
 namespace bn254 {
 using G1 = Group<GMSM_BN254_G1, 4, 1>;
 using G2 = Group<GMSM_BN254_G2, 4, 2>;
@@ -123,6 +140,7 @@ using G1Affine = G1::Affine;
 using G1Jac = G1::Jac;
 using G2Affine = G2::Affine;
 using G2Jac = G2::Jac;
+GMSM_HOST_TO_LAGRANGE
 }  // namespace bn254
 namespace bls12381 {
 using G1 = Group<GMSM_BLS12381_G1, 6, 1>;
@@ -131,6 +149,7 @@ using G1Affine = G1::Affine;
 using G1Jac = G1::Jac;
 using G2Affine = G2::Affine;
 using G2Jac = G2::Jac;
+GMSM_HOST_TO_LAGRANGE
 }  // namespace bls12381
 namespace bls12377 {   // ecc/bls12-377
 using G1 = Group<GMSM_BLS12377_G1, 6, 1>;
@@ -139,6 +158,7 @@ using G1Affine = G1::Affine;
 using G1Jac = G1::Jac;
 using G2Affine = G2::Affine;
 using G2Jac = G2::Jac;
+GMSM_HOST_TO_LAGRANGE
 }  // namespace bls12377
 namespace secp256k1 {   // ecc/secp256k1 (G1 only)
 using G1 = Group<GMSM_SECP256K1_G1, 4, 1>;
@@ -152,16 +172,19 @@ using G1Affine = G1::Affine;
 using G1Jac = G1::Jac;
 using G2Affine = G2::Affine;
 using G2Jac = G2::Jac;
+GMSM_HOST_TO_LAGRANGE
 }  // namespace bw6761
 namespace bls24315 {   // ecc/bls24-315 (G1; G2 is over Fp4 and stays on the CPU path)
 using G1 = Group<GMSM_BLS24315_G1, 5, 1>;
 using G1Affine = G1::Affine;
 using G1Jac = G1::Jac;
+GMSM_HOST_TO_LAGRANGE
 }  // namespace bls24315
 namespace bls24317 {   // ecc/bls24-317 (G1)
 using G1 = Group<GMSM_BLS24317_G1, 5, 1>;
 using G1Affine = G1::Affine;
 using G1Jac = G1::Jac;
+GMSM_HOST_TO_LAGRANGE
 }  // namespace bls24317
 namespace bw6633 {   // ecc/bw6-633: both groups over the 10-word Fp, fr.Element = [5]uint64
 using G1 = Group<GMSM_BW6633_G1, 10, 1, 5>;
@@ -170,6 +193,9 @@ using G1Affine = G1::Affine;
 using G1Jac = G1::Jac;
 using G2Affine = G2::Affine;
 using G2Jac = G2::Jac;
+GMSM_HOST_TO_LAGRANGE
 }  // namespace bw6633
+
+#undef GMSM_HOST_TO_LAGRANGE
 
 }  // namespace gmsm_host
