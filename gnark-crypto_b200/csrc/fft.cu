@@ -18,6 +18,7 @@
 //   eval                          ecc/bn254/kzg/kzg.go:55-63
 //   dividePolyByXminusA           ecc/bn254/kzg/kzg.go:567-582
 //   the gamma-fold of BatchOpenSinglePoint   ecc/bn254/kzg/kzg.go:302-319
+//   the strided linear combinations of shplonk.BatchOpen / fflonk.Fold (gmsm_fr_poly_lincomb_device)
 #include <cuda_runtime.h>
 
 #include <cstdio>
@@ -353,6 +354,19 @@ extern "C" int gmsm_fr_poly_div_x_minus_a_device(int fr_field, const void* d_f, 
   });
 }
 
+// launch(batch, accumulate, strided) of poly_lincomb_schedule: k_poly_fold over d_out[0, out_len) on `stream`
+template <class P>
+auto poly_fold_launcher(void* d_out, size_t out_len, void* stream) {
+  const unsigned blocks = (unsigned)std::min<uint64_t>((out_len + 255) / 256, GMSM_NUM_SMS * 32u);
+  return [=](const PolyFoldBatch<P>& b, int accumulate, bool strided) {
+    Fp<P>* out = reinterpret_cast<Fp<P>*>(d_out);
+    if (strided)
+      k_poly_fold<P, true><<<blocks, 256, 0, (cudaStream_t)stream>>>(out, out_len, b, accumulate);
+    else
+      k_poly_fold<P, false><<<blocks, 256, 0, (cudaStream_t)stream>>>(out, out_len, b, accumulate);
+  };
+}
+
 extern "C" int gmsm_fr_poly_fold_device(int fr_field, const void* const* d_polys, const size_t* lens, size_t k, const uint64_t* gamma,
                                         void* d_out, size_t out_len, void* stream) {
   if (!gmsm_fft_fr_bytes(fr_field)) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
@@ -372,6 +386,37 @@ extern "C" int gmsm_fr_poly_fold_device(int fr_field, const void* const* d_polys
     poly_fold_schedule<P>(reinterpret_cast<const F* const*>(d_polys), len.data(), k, g, [&](const PolyFoldBatch<P>& b, int accumulate) {
       k_poly_fold<P><<<blocks, 256, 0, st>>>(reinterpret_cast<F*>(d_out), out_len, b, accumulate);
     });
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fr_poly_lincomb_device(int fr_field, const void* const* d_polys, const size_t* lens, const uint64_t* scalars,
+                                           const size_t* strides, const size_t* offsets, size_t k, void* d_out, size_t out_len,
+                                           int accumulate, void* stream) {
+  const size_t fb = gmsm_fft_fr_bytes(fr_field);
+  if (!fb) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (k == 0 || out_len == 0) return set_err(GMSM_EINVAL, "nothing to combine (k = %zu, out_len = %zu)", k, out_len);
+  if (!d_polys || !lens || !scalars || !strides || !offsets || !d_out) return set_err(GMSM_EINVAL, "null argument");
+  const uintptr_t o0 = (uintptr_t)d_out, o1 = o0 + out_len * fb;
+  for (size_t i = 0; i < k; i++) {
+    if (strides[i] == 0) return set_err(GMSM_EINVAL, "stride of polynomial %zu is 0", i);
+    if (!lens[i]) continue;
+    if (!d_polys[i]) return set_err(GMSM_EINVAL, "polynomial %zu is null", i);
+    const uintptr_t p0 = (uintptr_t)d_polys[i], p1 = p0 + lens[i] * fb;
+    if (p0 < o1 && o0 < p1) return set_err(GMSM_EINVAL, "polynomial %zu overlaps the output", i);
+  }
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    std::vector<F> s(k);
+    for (size_t i = 0; i < k; i++) {
+      memcpy(s[i].l, scalars + i * (fb / 8), sizeof(F));
+      if (!host_is_reduced(s[i])) return set_err(GMSM_EINVAL, "scalar %zu is not a reduced fr.Element", i);
+    }
+    std::vector<uint64_t> len(lens, lens + k), str(strides, strides + k), off(offsets, offsets + k);
+    poly_lincomb_schedule<P>(reinterpret_cast<const F* const*>(d_polys), len.data(), s.data(), str.data(), off.data(), k,
+                             accumulate ? 1 : 0, poly_fold_launcher<P>(d_out, out_len, stream));
     CK(cudaGetLastError());
     return GMSM_OK;
   });

@@ -1,6 +1,7 @@
-// Device side of the Fr polynomial steps of kzg.Open and kzg.BatchOpenSinglePoint: evaluation, division by (X - a) and the
-// gamma-fold.  Reference: eval (ecc/bn254/kzg/kzg.go:55-63), dividePolyByXminusA (:567-582), the fold of BatchOpenSinglePoint
-// (:302-319); the kzg packages of the other pairing curves are the same generated code.  In a header of their own, like
+// Device side of the Fr polynomial steps of kzg.Open, kzg.BatchOpenSinglePoint and the SHPLONK / FFLONK batch openings:
+// evaluation, division by (X - a) and the strided linear combination, of which the gamma-fold is the stride-1 case.  Reference:
+// eval (ecc/bn254/kzg/kzg.go:55-63), dividePolyByXminusA (:567-582), the fold of BatchOpenSinglePoint (:302-319); the kzg
+// packages of the other pairing curves are the same generated code.  In a header of their own, like
 // fft_kernels.cuh, so that the CPU kernel emulation of tests/emu/ compiles and runs them too (tests/test_emu_poly_cpu.py);
 // fft.cu includes this file and holds the entry points.  The launch schedules below are shared by both.
 //
@@ -140,24 +141,37 @@ __global__ void k_poly_write(const Fp<P>* x, uint64_t m, PolyMults<P> mu, int lo
   if (fa && blockIdx.x == 0 && tid == 0) store_vec(fa, load_vec(s));
 }
 
-// one batch of the fold: out[j] (+)= sum_i g[i] p[i][j] over the polynomials with j < len[i]
+// one batch of the linear combination: out[m stride[i] + offset[i]] (+)= g[i] p[i][m] for m < len[i].  stride and offset follow
+// the fields of the stride-1 fold so that its kernel reads its parameters where it always did.
 template <class P>
 struct PolyFoldBatch {
   const Fp<P>* p[POLY_FOLD_BATCH];
   uint64_t len[POLY_FOLD_BATCH];
   Fp<P> g[POLY_FOLD_BATCH];
   int count;
+  uint64_t stride[POLY_FOLD_BATCH];
+  uint64_t offset[POLY_FOLD_BATCH];
 };
 
-// fold: out[j] = sum_i gamma^i f_i[j] for j < out_len, every input read once, out written once per batch of POLY_FOLD_BATCH
-// polynomials (accumulate != 0: add to out).  Grid-stride, no barrier.
-template <class P>
+// linear combination: out[j] = sum_i g[i] p[i][(j - offset[i]) / stride[i]] for j < out_len, over the inputs whose stride divides
+// j - offset[i] (j >= offset[i]) with a quotient below len[i]; every input read once, out written once per batch of
+// POLY_FOLD_BATCH inputs (accumulate != 0: add to out).  Grid-stride, no barrier.  STRIDED = false: every stride is 1 and every
+// offset 0 (the gamma-fold), and the index arithmetic reduces to j < len[i].
+template <class P, bool STRIDED = false>
 __global__ void k_poly_fold(Fp<P>* __restrict__ out, uint64_t out_len, PolyFoldBatch<P> b, int accumulate) {
   for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < out_len; j += (uint64_t)gridDim.x * blockDim.x) {
     Fp<P> acc = accumulate ? load_vec(out + j) : Fp<P>::zero();
 #pragma unroll
-    for (int i = 0; i < POLY_FOLD_BATCH; i++)
-      if (i < b.count && j < b.len[i]) acc = fp_add(acc, fp_mul(load_vec(b.p[i] + j), b.g[i]));
+    for (int i = 0; i < POLY_FOLD_BATCH; i++) {
+      if (i >= b.count) continue;
+      if constexpr (STRIDED) {
+        if (j < b.offset[i]) continue;
+        const uint64_t d = j - b.offset[i], m = d / b.stride[i];
+        if (m * b.stride[i] == d && m < b.len[i]) acc = fp_add(acc, fp_mul(load_vec(b.p[i] + m), b.g[i]));
+      } else {
+        if (j < b.len[i]) acc = fp_add(acc, fp_mul(load_vec(b.p[i] + j), b.g[i]));
+      }
+    }
     store_vec(out + j, acc);
   }
 }
@@ -223,21 +237,37 @@ void poly_div_schedule(const Fp<P>* f, uint64_t n, const Fp<P>& a, Fp<P>* h, Fp<
           tiles(l));
 }
 
-// out = sum_i gamma^i polys[i] (zero past lens[i]); launch(batch, accumulate) runs k_poly_fold
+// out (+)= sum_i scalars[i] polys[i] placed at stride strides[i] from offsets[i] (strides / offsets NULL: 1 / 0); launch(batch,
+// accumulate, strided) runs k_poly_fold<P, strided>, strided = false for a batch whose strides are all 1 and offsets all 0
 template <class P, class Launch>
-void poly_fold_schedule(const Fp<P>* const* polys, const uint64_t* lens, uint64_t k, const Fp<P>& gamma, Launch&& launch) {
-  Fp<P> g = Fp<P>::one();
+void poly_lincomb_schedule(const Fp<P>* const* polys, const uint64_t* lens, const Fp<P>* scalars, const uint64_t* strides,
+                           const uint64_t* offsets, uint64_t k, int accumulate, Launch&& launch) {
   for (uint64_t i0 = 0; i0 < k; i0 += POLY_FOLD_BATCH) {
     PolyFoldBatch<P> b{};
     b.count = (int)(k - i0 < (uint64_t)POLY_FOLD_BATCH ? k - i0 : POLY_FOLD_BATCH);
+    bool strided = false;
     for (int i = 0; i < b.count; i++) {
       b.p[i] = polys[i0 + i];
       b.len[i] = lens[i0 + i];
-      b.g[i] = g;
-      g = fp_mul(g, gamma);
+      b.g[i] = scalars[i0 + i];
+      b.stride[i] = strides ? strides[i0 + i] : 1;
+      b.offset[i] = offsets ? offsets[i0 + i] : 0;
+      strided |= b.stride[i] != 1 || b.offset[i] != 0;
     }
-    launch(b, i0 > 0 ? 1 : 0);
+    launch(b, i0 > 0 ? 1 : accumulate, strided);
   }
+}
+
+// out = sum_i gamma^i polys[i] (zero past lens[i]): the linear combination with scalars gamma^i, stride 1 and offset 0;
+// launch(batch, accumulate) runs k_poly_fold<P, false>
+template <class P, class Launch>
+void poly_fold_schedule(const Fp<P>* const* polys, const uint64_t* lens, uint64_t k, const Fp<P>& gamma, Launch&& launch) {
+  if (k == 0) return;
+  std::vector<Fp<P>> g(k);
+  g[0] = Fp<P>::one();
+  for (uint64_t i = 1; i < k; i++) g[i] = fp_mul(g[i - 1], gamma);
+  poly_lincomb_schedule<P>(polys, lens, g.data(), nullptr, nullptr, k, 0,
+                           [&](const PolyFoldBatch<P>& b, int accumulate, bool) { launch(b, accumulate); });
 }
 
 }  // namespace

@@ -26,6 +26,7 @@ import numpy as np
 from . import _native
 from .fft import _FIELDS
 from .multiexp import CURVES, BatchScalarMultiplication, MultiExpConfig, MultiExpError, ResidentBases, _check, _words
+from .transcript import Transcript
 
 MARKER = 0xDEADBEEF  # utils/unsafe/dump_slice.go:78
 
@@ -278,6 +279,15 @@ class _DevicePoly:
         _check(_native.lib().gmsm_fr_poly_fold_device(self.field, ptrs, ln.ctypes.data, len(d_polys), gamma.ctypes.data, d_out.data_ptr(),
                                                        out_len, self.stream))
 
+    def lincomb(self, d_polys, lens, scalars: np.ndarray, strides, offsets, d_out, out_len: int, accumulate: bool = False):
+        """d_out[m * strides[i] + offsets[i]] (+)= scalars[i] * d_polys[i][m]; scalars: (k, fr.Limbs) reduced limbs"""
+        k = len(d_polys)
+        ptrs = (ctypes.c_void_p * k)(*[d.data_ptr() for d in d_polys])
+        ln, st, off = (np.array(v, dtype=np.uint64) for v in (lens, strides, offsets))
+        sc = np.ascontiguousarray(scalars, dtype=np.uint64)
+        _check(_native.lib().gmsm_fr_poly_lincomb_device(self.field, ptrs, ln.ctypes.data, sc.ctypes.data, st.ctypes.data, off.ctypes.data,
+                                                          k, d_out.data_ptr(), out_len, 1 if accumulate else 0, self.stream))
+
 
 @dataclass
 class OpeningProof:
@@ -495,16 +505,15 @@ def derive_gamma(point, digests, claimed_values, hf, curve: str, *data_transcrip
     c = curve.split("_")[0]
     cp = CURVE_PARAMS[c]
     r = cp.r
-    h = hf()
-    h.update(b"gamma")
-    h.update(_fr_marshal(point, r))
+    fs = Transcript(hf, "gamma")
+    fs.Bind("gamma", _fr_marshal(point, r))
     for d in digests:
-        h.update(g1_raw_bytes(d, c))
+        fs.Bind("gamma", g1_raw_bytes(d, c))
     for v in np.ascontiguousarray(claimed_values, dtype=np.uint64).reshape(-1, cp.fr_words):
-        h.update(_fr_marshal(v, r))
+        fs.Bind("gamma", _fr_marshal(v, r))
     for b in data_transcript:
-        h.update(b)
-    return int.from_bytes(h.digest(), "big") % r
+        fs.Bind("gamma", b)
+    return int.from_bytes(fs.ComputeChallenge("gamma"), "big") % r
 
 
 def BatchOpenSinglePoint(polynomials, digests, point: np.ndarray, hf, pk: ProvingKey, *data_transcript: bytes) -> BatchOpeningProof:

@@ -241,6 +241,15 @@ int gmsm_fr_poly_div_x_minus_a_device(int fr_field, const void* d_f, size_t n, c
  * pointers, each input read once */
 int gmsm_fr_poly_fold_device(int fr_field, const void* const* d_polys, const size_t* lens, size_t k, const uint64_t* gamma,
                              void* d_out, size_t out_len, void* stream);
+/* linear combination of the SHPLONK / FFLONK batch openings (ecc/bn254/shplonk, ecc/bn254/fflonk):
+ * d_out[m * strides[i] + offsets[i]] (+)= scalars[i] * f_i[m] for m < lens[i], summed over i, for the indices below out_len; every
+ * other index of d_out[0, out_len) is set to 0 (accumulate = 0) or left as it is (accumulate != 0).  scalars: k x fr.Limbs u64,
+ * reduced.  The gamma-fold is scalars gamma^i, strides 1, offsets 0; stride t with offsets 0..t-1 interleaves t polynomials
+ * (fflonk.Fold).  GMSM_EINVAL: unknown field, k = 0, out_len = 0, a zero stride, an unreduced scalar, an input overlapping
+ * d_out. */
+int gmsm_fr_poly_lincomb_device(int fr_field, const void* const* d_polys, const size_t* lens, const uint64_t* scalars,
+                                const size_t* strides, const size_t* offsets, size_t k, void* d_out, size_t out_len, int accumulate,
+                                void* stream);
 
 /* ---- kzg.ToLagrangeG1 (ecc/bn254/kzg/utils.go:25-64; the same for the other pairing curves): the canonical SRS [tau^i]G in,
  * its Lagrange form [L_i(tau)]G out, by an inverse FFT over G1 points on the device.  Curves: the G1 groups of bn254, bls12-381,
