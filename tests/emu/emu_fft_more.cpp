@@ -13,8 +13,9 @@ namespace {
 // the dynamic shared memory of k_fft_tile (`extern __shared__ smem_raw[]`): 1024 elements of up to 48 bytes
 thread_local __attribute__((aligned(16))) unsigned char smem_raw[TILE * 48];
 
+// count > 1: the same transform on count consecutive n-element vectors, one domain build for all of them
 template <class P>
-int emu_fft(uint32_t* a_words, uint64_t n, int logn, int inverse, int decimation, int coset, const uint32_t* consts5) {
+int emu_fft(uint32_t* a_words, uint64_t n, int logn, int inverse, int decimation, int coset, const uint32_t* consts5, uint64_t count = 1) {
   using F = Fp<P>;
   static_assert(sizeof(F) <= 48, "smem_raw holds 1024 elements of at most 48 bytes");
   constexpr int N = P::N;   // u32 limbs per element: consts5 is 5 rows of N
@@ -34,34 +35,44 @@ int emu_fft(uint32_t* a_words, uint64_t n, int logn, int inverse, int decimation
   if (half) emu_launch(k_fft_powers<P>, dim3(grid(half)), 256u, tw.data(), half, (const F*)(pw.data() + 128), logn > 0 ? logn - 1 : 0);
   // run_fft
   const F one = F::one();
-  if (!inverse && coset) emu_launch(k_fft_scale<P>, dim3(grid(n)), 256u, a, n, logn, (const F*)pw.data(), 1, (int)(decimation == 0), one, 0);
-  if (n > 1) {
-    const uint32_t tile = (uint32_t)std::min<uint64_t>(n, TILE);
-    if (decimation == 1) {
-      for (uint64_t h = half; h >= tile; h >>= 1) emu_launch(k_fft_dif_stage<P>, dim3(grid(half)), 256u, a, (const F*)tw.data(), half, h, half / h);
-      emu_launch_coop(k_fft_tile<P, true>, dim3((unsigned)(n / tile)), tile / 2, a, (const F*)tw.data(), n, tile);
-    } else {
-      emu_launch_coop(k_fft_tile<P, false>, dim3((unsigned)(n / tile)), tile / 2, a, (const F*)tw.data(), n, tile);
-      for (uint64_t h = tile; h <= half; h <<= 1) emu_launch(k_fft_dit_stage<P>, dim3(grid(half)), 256u, a, (const F*)tw.data(), half, h, half / h);
+  for (uint64_t s = 0; s < count; s++, a += n) {
+    if (!inverse && coset) emu_launch(k_fft_scale<P>, dim3(grid(n)), 256u, a, n, logn, (const F*)pw.data(), 1, (int)(decimation == 0), one, 0);
+    if (n > 1) {
+      const uint32_t tile = (uint32_t)std::min<uint64_t>(n, TILE);
+      if (decimation == 1) {
+        for (uint64_t h = half; h >= tile; h >>= 1) emu_launch(k_fft_dif_stage<P>, dim3(grid(half)), 256u, a, (const F*)tw.data(), half, h, half / h);
+        emu_launch_coop(k_fft_tile<P, true>, dim3((unsigned)(n / tile)), tile / 2, a, (const F*)tw.data(), n, tile);
+      } else {
+        emu_launch_coop(k_fft_tile<P, false>, dim3((unsigned)(n / tile)), tile / 2, a, (const F*)tw.data(), n, tile);
+        for (uint64_t h = tile; h <= half; h <<= 1) emu_launch(k_fft_dit_stage<P>, dim3(grid(half)), 256u, a, (const F*)tw.data(), half, h, half / h);
+      }
     }
+    if (inverse) emu_launch(k_fft_scale<P>, dim3(grid(n)), 256u, a, n, logn, (const F*)(pw.data() + 64), coset ? 1 : 0, (int)(decimation == 1), card_inv, 1);
   }
-  if (inverse) emu_launch(k_fft_scale<P>, dim3(grid(n)), 256u, a, n, logn, (const F*)(pw.data() + 64), coset ? 1 : 0, (int)(decimation == 1), card_inv, 1);
   return 0;
 }
 }  // namespace
 
 // field: GMSM_FR_* (0 bn254, 1 bls12-381, 2 bls12-377, 3 bls24-315, 4 bls24-317, 5 bw6-633, 6 bw6-761); a: n elements of
 // fr.Limbs u64 (8 / 10 / 12 u32) Montgomery limbs, transformed in place; consts5: 5 such elements
-extern "C" int emu_fft_more_run(int field, uint32_t* a, uint64_t n, int logn, int inverse, int decimation, int coset, const uint32_t* consts5) {
+// the transform of emu_fft_more_run on each of `count` consecutive n-element vectors of a (the domain built once)
+extern "C" int emu_fft_more_run_many(int field, uint32_t* a, uint64_t count, uint64_t n, int logn, int inverse, int decimation, int coset,
+                                     const uint32_t* consts5) {
   if (n == 0 || (n & (n - 1)) || (1ull << logn) != n) return 1;
   switch (field) {
-    case 0: return emu_fft<bn254_fr>(a, n, logn, inverse, decimation, coset, consts5);
-    case 1: return emu_fft<bls12381_fr>(a, n, logn, inverse, decimation, coset, consts5);
-    case 2: return emu_fft<bls12377_fr>(a, n, logn, inverse, decimation, coset, consts5);
-    case 3: return emu_fft<bls24315_fr>(a, n, logn, inverse, decimation, coset, consts5);
-    case 4: return emu_fft<bls24317_fr>(a, n, logn, inverse, decimation, coset, consts5);
-    case 5: return emu_fft<bw6633_fr>(a, n, logn, inverse, decimation, coset, consts5);
-    case 6: return emu_fft<bw6761_fr>(a, n, logn, inverse, decimation, coset, consts5);
+    case 0: return emu_fft<bn254_fr>(a, n, logn, inverse, decimation, coset, consts5, count);
+    case 1: return emu_fft<bls12381_fr>(a, n, logn, inverse, decimation, coset, consts5, count);
+    case 2: return emu_fft<bls12377_fr>(a, n, logn, inverse, decimation, coset, consts5, count);
+    case 3: return emu_fft<bls24315_fr>(a, n, logn, inverse, decimation, coset, consts5, count);
+    case 4: return emu_fft<bls24317_fr>(a, n, logn, inverse, decimation, coset, consts5, count);
+    case 5: return emu_fft<bw6633_fr>(a, n, logn, inverse, decimation, coset, consts5, count);
+    case 6: return emu_fft<bw6761_fr>(a, n, logn, inverse, decimation, coset, consts5, count);
   }
   return 1;
+}
+
+// field: GMSM_FR_* (0 bn254, 1 bls12-381, 2 bls12-377, 3 bls24-315, 4 bls24-317, 5 bw6-633, 6 bw6-761); a: n elements of
+// fr.Limbs u64 (8 / 10 / 12 u32) Montgomery limbs, transformed in place; consts5: 5 such elements
+extern "C" int emu_fft_more_run(int field, uint32_t* a, uint64_t n, int logn, int inverse, int decimation, int coset, const uint32_t* consts5) {
+  return emu_fft_more_run_many(field, a, 1, n, logn, inverse, decimation, coset, consts5);
 }
