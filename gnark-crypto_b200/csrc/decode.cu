@@ -62,27 +62,18 @@ extern "C" int gmsm_g1_decode_device(gmsm_curve_t curve, const void* d_bytes, si
 extern "C" int gmsm_g1_decode(gmsm_curve_t curve, const uint8_t* bytes, size_t n, int raw, int check_on_curve, uint64_t* out_points) {
   size_t ab = gmsm_affine_bytes(curve);
   if (!ab) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) return set_err(GMSM_ENODEV, "no CUDA device (%s); this engine has no CPU fallback", cudaGetErrorString(e));
+  if (int rc = use_device(default_device())) return rc;
   if (n == 0) return GMSM_OK;
-  int device = 0;
-  if (const char* ev = getenv("GMSM_DEVICE")) device = atoi(ev);
-  CK(cudaSetDevice(device));
   const size_t in_bytes = n * (raw ? ab : ab / 2);
-  void *d_in = nullptr, *d_out = nullptr, *d_err = nullptr;
-  auto cleanup = [&]() { cudaFree(d_in); cudaFree(d_out); cudaFree(d_err); };
-  if (cudaMalloc(&d_in, in_bytes) != cudaSuccess || cudaMalloc(&d_out, n * ab) != cudaSuccess || cudaMalloc(&d_err, 8) != cudaSuccess) {
-    cleanup();
+  DevBuf d_in, d_out, d_err;
+  if (cudaMalloc(&d_in.p, in_bytes) != cudaSuccess || cudaMalloc(&d_out.p, n * ab) != cudaSuccess || cudaMalloc(&d_err.p, 8) != cudaSuccess)
     return set_err(GMSM_ENOMEM, "gmsm_g1_decode: device allocation failed");
-  }
   int rc = GMSM_OK;
   unsigned long long first = ~0ull;
-  cudaError_t ce = cudaMemcpy(d_in, bytes, in_bytes, cudaMemcpyHostToDevice);
-  if (ce == cudaSuccess) rc = gmsm_g1_decode_device(curve, d_in, n, raw, check_on_curve, d_out, d_err, nullptr);
-  if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpy(out_points, d_out, n * ab, cudaMemcpyDeviceToHost);
-  if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpy(&first, d_err, 8, cudaMemcpyDeviceToHost);
-  cleanup();
+  cudaError_t ce = cudaMemcpy(d_in.p, bytes, in_bytes, cudaMemcpyHostToDevice);
+  if (ce == cudaSuccess) rc = gmsm_g1_decode_device(curve, d_in.p, n, raw, check_on_curve, d_out.p, d_err.p, nullptr);
+  if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpy(out_points, d_out.p, n * ab, cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpy(&first, d_err.p, 8, cudaMemcpyDeviceToHost);
   if (ce != cudaSuccess) return set_err(GMSM_ECUDA, "gmsm_g1_decode: %s", cudaGetErrorString(ce));
   if (rc != GMSM_OK) return rc;
   if (first != ~0ull) return set_err(GMSM_EINVAL, "point %llu: %s", first >> 8, dec_message((int)(first & 0xFF)));

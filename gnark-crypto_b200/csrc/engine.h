@@ -31,6 +31,18 @@ struct CurveInfo {
   int scalar_bytes; // one fr.Element: 32 (4 x uint64), 48 for bw6-761 (6 x uint64)
 };
 
+// GMSM_ENODEV when the process sees no CUDA device; GMSM_EINVAL with range_fmt (given the id and the device count) when
+// `device` is not one of them; otherwise `device` is made current (gmsm.cu)
+int use_device(int device, const char* range_fmt = "device %d out of range (%d devices)");
+// the device of the entry points that take none: GMSM_DEVICE, default 0
+int default_device();
+
+struct DevBuf {   // a device allocation freed on every exit path (the CK macro returns early on errors)
+  void* p = nullptr;
+  ~DevBuf() { if (p) cudaFree(p); }
+  template <class T> T* as() { return reinterpret_cast<T*>(p); }
+};
+
 }  // namespace gmsm
 
 struct gmsm_ctx {
@@ -100,7 +112,6 @@ struct gmsm_ctx {
   // completion of the last call enqueued on this context: every device-level entry point makes its stream wait for it
   // before touching the shared workspace, so calls from different streams / threads queue up instead of overlapping
   cudaEvent_t ev_done = nullptr;
-  float stage_ms[8] = {};
   bool have_stage = false;
   std::mutex mu;
 };
@@ -129,6 +140,7 @@ static inline unsigned nblk(size_t n, unsigned t) { return (unsigned)((n + t - 1
 // one table per (curve, group); each lives in its own translation unit (inst_*.cu) so the four
 // heavy template instantiations compile in parallel
 struct GroupVTable {
+  CurveInfo ci;   // the sizes of the group's types (GMSM_INSTANTIATE)
   int (*window_sums)(gmsm_ctx*, const void* d_points, const void* d_scalars, size_t n, void* d_partials, cudaStream_t);
   int (*accumulate)(gmsm_ctx*, const void* d_points, const void* d_scalars, size_t n, int rmw, cudaStream_t);
   int (*bucket_reduce)(gmsm_ctx*, void* d_partials, cudaStream_t);

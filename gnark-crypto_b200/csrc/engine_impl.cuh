@@ -81,40 +81,28 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
   }
   const uint32_t range_sz = c->shared ? (p.nb_total + (uint32_t)NPASS - 1) / (uint32_t)NPASS : p.nb;
   const int SPLIT_W = (!c->affine && sizeof(F) <= 48 && p.nwin >= 6 && n >= (1u << 16)) ? std::min(c->shared ? c->split_tab : c->split_w, NPASS) : NPASS;
-  if (c->shared) {
-    unsigned blocks = std::min<unsigned>(nblk(n, 256 * 4), GMSM_NUM_SMS * 2u);
-    auto scatter = [&](int r, cudaStream_t s) {
+  const unsigned scatter_blocks = std::min<unsigned>(nblk(n, 256 * 4), GMSM_NUM_SMS * (c->shared ? 2u : 8u));
+  auto scatter = [&](int r, cudaStream_t s) {   // pass r: bucket range r (window-table mode) or window r
+    if (c->shared) {
       const uint32_t blo = std::min<uint64_t>((uint64_t)r * range_sz, p.nb_total);
       const uint32_t bhi = std::min<uint64_t>((uint64_t)(r + 1) * range_sz, p.nb_total);
       if (blo >= bhi) return;
-      k_scatter_shared<<<dim3(blocks, (unsigned)p.nwin), 256, 0, s>>>(c->digits, c->ranks, n32, c->tab_stride, c->hist, c->offsets,
-                                                                       c->entries, blo, bhi, c->hist + nbp + 4);
-      launches++;
-    };
-    if (SPLIT_W < NPASS) {
-      CK(cudaEventRecord(c->ev_split[0], st));
-      CK(cudaStreamWaitEvent(c->aux, c->ev_split[0], 0));
-      for (int r = SPLIT_W; r < NPASS; r++) scatter(r, c->aux);
-      CK(cudaEventRecord(c->ev_split[1], c->aux));
+      k_scatter_shared<<<dim3(scatter_blocks, (unsigned)p.nwin), 256, 0, s>>>(c->digits, c->ranks, n32, c->tab_stride, c->hist,
+                                                                               c->offsets, c->entries, blo, bhi, c->hist + nbp + 4);
+    } else {
+      k_scatter_window<<<scatter_blocks, 256, 0, s>>>(c->digits + (size_t)r * n, c->ranks + (size_t)r * n, n32, c->hist + (size_t)r * p.nb,
+                                                      c->offsets + (size_t)r * p.nb, c->entries, c->hist + nbp + 4);
     }
-    for (int r = 0; r < SPLIT_W; r++) scatter(r, st);
-    LAUNCH_CHECK();
-  } else {
-    unsigned blocks = std::min<unsigned>(nblk(n, 256 * 4), GMSM_NUM_SMS * 8u);
-    auto scatter = [&](int j, cudaStream_t s) {
-      k_scatter_window<<<blocks, 256, 0, s>>>(c->digits + (size_t)j * n, c->ranks + (size_t)j * n, n32, c->hist + (size_t)j * p.nb,
-                                              c->offsets + (size_t)j * p.nb, c->entries, c->hist + nbp + 4);
-      launches++;
-    };
-    if (SPLIT_W < NPASS) {
-      CK(cudaEventRecord(c->ev_split[0], st));           // scan done: offsets, digits, hist are ready
-      CK(cudaStreamWaitEvent(c->aux, c->ev_split[0], 0));
-      for (int j = SPLIT_W; j < p.nwin; j++) scatter(j, c->aux);
-      CK(cudaEventRecord(c->ev_split[1], c->aux));
-    }
-    for (int j = 0; j < SPLIT_W; j++) scatter(j, st);
-    LAUNCH_CHECK();
+    launches++;
+  };
+  if (SPLIT_W < NPASS) {
+    CK(cudaEventRecord(c->ev_split[0], st));           // scan done: offsets, digits, hist are ready
+    CK(cudaStreamWaitEvent(c->aux, c->ev_split[0], 0));
+    for (int r = SPLIT_W; r < NPASS; r++) scatter(r, c->aux);
+    CK(cudaEventRecord(c->ev_split[1], c->aux));
   }
+  for (int r = 0; r < SPLIT_W; r++) scatter(r, st);
+  LAUNCH_CHECK();
   mark(3);
   if (c->affine && c->shared) return set_err(GMSM_EINVAL, "internal: window tables need the default accumulation mode");
   if (c->affine && rmw) return set_err(GMSM_EINVAL, "internal: batch-affine accumulation cannot extend existing buckets");
@@ -134,7 +122,6 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
     const uint32_t* off_cur = c->offsets;
     const A* src_cur = nullptr;
     size_t m_up = n * (size_t)p.nwin;
-    const size_t fe = sizeof(F);
     F* bp = reinterpret_cast<F*>(c->aff_bp);
     const size_t bp_stride = c->aff_tcap / 1024 + 8;
     for (int l = 0; l < nlevels; l++) {
@@ -170,7 +157,6 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
       src_cur = dst;
       off_cur = off_next;
       m_up = m_next;
-      (void)fe;
     }
     if (nlevels == 0)
       k_aff_to_buckets<G, true><<<std::min<unsigned>(nblk(nbt, 256), GMSM_NUM_SMS * 8u), 256, 0, st>>>(points, c->entries, src_cur, off_cur, nbt, buckets);
@@ -379,12 +365,13 @@ static int run_to_lagrange(const void* d_points, size_t n, const uint64_t* w_inv
   return GMSM_OK;
 }
 
+#define GMSM_CURVE_INFO(G) {G::F::N, G::FrParams::BITS, 4 * G::FrParams::N}
 #define GMSM_INSTANTIATE(G, NAME)                                                                  \
-  const GroupVTable NAME = {&run_window_sums<G>, &run_accumulate<G>, &run_bucket_reduce<G>, &run_finalize<G>, &run_generate<G>, &test_op_sizes<G>, \
-                            &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>};
+  const GroupVTable NAME = {GMSM_CURVE_INFO(G), &run_window_sums<G>, &run_accumulate<G>, &run_bucket_reduce<G>, &run_finalize<G>, &run_generate<G>, \
+                            &test_op_sizes<G>, &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>};
 // the G1 groups of the seven pairing curves: also kzg.ToLagrangeG1
 #define GMSM_INSTANTIATE_PAIRING_G1(G, NAME)                                                       \
-  const GroupVTable NAME = {&run_window_sums<G>, &run_accumulate<G>, &run_bucket_reduce<G>, &run_finalize<G>, &run_generate<G>, &test_op_sizes<G>, \
-                            &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>, &run_to_lagrange<G>};
+  const GroupVTable NAME = {GMSM_CURVE_INFO(G), &run_window_sums<G>, &run_accumulate<G>, &run_bucket_reduce<G>, &run_finalize<G>, &run_generate<G>, \
+                            &test_op_sizes<G>, &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>, &run_to_lagrange<G>};
 
 }  // namespace gmsm

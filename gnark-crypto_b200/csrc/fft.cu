@@ -67,29 +67,32 @@ struct FrConsts {
   int max_order;      // maxOrderRoot, generator.go:24
   uint64_t mult_gen;  // GeneratorFullMultiplicativeGroup, fft/domain.go:55-63
 };
-const FrConsts FR_BN254 = {"19103219067921713944291392827692070036145651957329286315305642004821462161904", 28, 5};
-const FrConsts FR_BLS12381 = {"10238227357739495823651030575849232062558860180284477541189508159991286009131", 32, 7};
-// ecc/bls12-377/fr/generator.go:23-24, fr/fft/domain.go:59
-const FrConsts FR_BLS12377 = {"8065159656716812877374967518403273466521432693661810619979959746626482506078", 47, 22};
-// ecc/{bls24-315,bls24-317,bw6-633,bw6-761}/fr/generator.go:23-24, fr/fft/domain.go:59.  Each root is
-// GeneratorFullMultiplicativeGroup^((r - 1) >> maxOrderRoot), of order exactly 2^maxOrderRoot.
-const FrConsts FR_BLS24315 = {"1792993287828780812362846131493071959406149719416102105453370749552622525216", 22, 7};
-const FrConsts FR_BLS24317 = {"16532287748948254263922689505213135976137839535221842169193829039521719560631", 60, 7};
-const FrConsts FR_BW6633 = {"4991787701895089137426454739366935169846548798279261157172811661565882460884369603588700158257", 20, 13};
-const FrConsts FR_BW6761 = {
-    "32863578547254505029601261939868325669770508939375122462904745766352256812585773382134936404344547323199885654433", 46, 15};
+// one row per scalar field id (GMSM_FR_*), in the order of the ids
+const FrConsts FR_CONSTS[] = {
+    {"19103219067921713944291392827692070036145651957329286315305642004821462161904", 28, 5},     // bn254
+    {"10238227357739495823651030575849232062558860180284477541189508159991286009131", 32, 7},     // bls12-381
+    // ecc/bls12-377/fr/generator.go:23-24, fr/fft/domain.go:59
+    {"8065159656716812877374967518403273466521432693661810619979959746626482506078", 47, 22},
+    // ecc/{bls24-315,bls24-317,bw6-633,bw6-761}/fr/generator.go:23-24, fr/fft/domain.go:59.  Each root is
+    // GeneratorFullMultiplicativeGroup^((r - 1) >> maxOrderRoot), of order exactly 2^maxOrderRoot.
+    {"1792993287828780812362846131493071959406149719416102105453370749552622525216", 22, 7},      // bls24-315
+    {"16532287748948254263922689505213135976137839535221842169193829039521719560631", 60, 7},     // bls24-317
+    {"4991787701895089137426454739366935169846548798279261157172811661565882460884369603588700158257", 20, 13},   // bw6-633
+    {"32863578547254505029601261939868325669770508939375122462904745766352256812585773382134936404344547323199885654433", 46,
+     15},                                                                                           // bw6-761
+};
+static_assert(sizeof(FR_CONSTS) / sizeof(FR_CONSTS[0]) == GMSM_FR_BW6761 + 1, "one row per scalar field id");
 
-const FrConsts* fr_consts(int field) {
-  switch (field) {
-    case GMSM_FR_BN254: return &FR_BN254;
-    case GMSM_FR_BLS12381: return &FR_BLS12381;
-    case GMSM_FR_BLS12377: return &FR_BLS12377;
-    case GMSM_FR_BLS24315: return &FR_BLS24315;
-    case GMSM_FR_BLS24317: return &FR_BLS24317;
-    case GMSM_FR_BW6633: return &FR_BW6633;
-    case GMSM_FR_BW6761: return &FR_BW6761;
-  }
-  return nullptr;
+const FrConsts* fr_consts(int field) { return field >= 0 && field <= GMSM_FR_BW6761 ? &FR_CONSTS[field] : nullptr; }
+
+// log2 of ecc.NextPowerOfTwo(m) into *logn, refused past maxOrderRoot as fr.Generator refuses it (generator.go:29)
+int domain_log(const FrConsts& fc, uint64_t m, int* logn) {
+  int k = 0;
+  while (k <= fc.max_order && ((uint64_t)1 << k) < m) k++;
+  if (k > fc.max_order)
+    return set_err(GMSM_EINVAL, "m (%llu) is too big: the required root of unity does not exist", (unsigned long long)m);
+  *logn = k;
+  return GMSM_OK;
 }
 
 template <class P>
@@ -198,9 +201,7 @@ int gmsm::fr_domain_inverses(int fr_field, uint64_t n, uint64_t* w_inv, uint64_t
   const FrConsts* fcp = fr_consts(fr_field);
   if (!fcp) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
   int logn = 0;
-  while (((uint64_t)1 << logn) < n) logn++;
-  if (logn > fcp->max_order)
-    return set_err(GMSM_EINVAL, "m (%llu) is too big: the required root of unity does not exist", (unsigned long long)n);  // generator.go:29
+  if (int rc = domain_log(*fcp, n, &logn)) return rc;
   return with_fr(fr_field, [&](auto tag) -> int {
     using P = typename decltype(tag)::type;
     const Fp<P> wi = fp_inv(host_pow2k(host_from_decimal<P>(fcp->root), fcp->max_order - logn));
@@ -214,19 +215,11 @@ int gmsm::fr_domain_inverses(int fr_field, uint64_t n, uint64_t* w_inv, uint64_t
 extern "C" gmsm_fft_domain_t* gmsm_fft_domain_create(int fr_field, uint64_t m, const uint64_t* shift, int device) {
   const FrConsts* fcp = fr_consts(fr_field);
   if (!fcp) { set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field); return nullptr; }
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) { set_err(GMSM_ENODEV, "no CUDA device (%s); this engine has no CPU fallback", cudaGetErrorString(e)); return nullptr; }
-  if (device < 0 || device >= ndev) { set_err(GMSM_EINVAL, "device %d out of range", device); return nullptr; }
-  cudaSetDevice(device);
+  if (use_device(device, "device %d out of range") != GMSM_OK) return nullptr;
   const FrConsts& fc = *fcp;
-  uint64_t x = 1;
   int logn = 0;
-  while (x < m) { x <<= 1; logn++; }   // ecc.NextPowerOfTwo(m)
-  if (logn > fc.max_order) {
-    set_err(GMSM_EINVAL, "m (%llu) is too big: the required root of unity does not exist", (unsigned long long)m);  // generator.go:29
-    return nullptr;
-  }
+  if (domain_log(fc, m, &logn) != GMSM_OK) return nullptr;
+  const uint64_t x = (uint64_t)1 << logn;
   gmsm_fft_domain* d = new gmsm_fft_domain();
   d->field = fr_field; d->device = device; d->n = x; d->logn = logn;
   d->words = (int)(gmsm_fft_fr_bytes(fr_field) / 8);
@@ -245,12 +238,8 @@ extern "C" void gmsm_fft_domain_free(gmsm_fft_domain_t* d) {
 }
 
 extern "C" size_t gmsm_fft_fr_bytes(int fr_field) {
-  switch (fr_field) {
-    case GMSM_FR_BN254: case GMSM_FR_BLS12381: case GMSM_FR_BLS12377: case GMSM_FR_BLS24315: case GMSM_FR_BLS24317: return 32;
-    case GMSM_FR_BW6633: return 40;
-    case GMSM_FR_BW6761: return 48;
-  }
-  return 0;
+  if (!fr_consts(fr_field)) return 0;   // (with_fr would set an error)
+  return (size_t)with_fr(fr_field, [](auto tag) { return (int)sizeof(Fp<typename decltype(tag)::type>); });
 }
 
 extern "C" uint64_t gmsm_fft_domain_cardinality(const gmsm_fft_domain_t* d) { return d ? d->n : 0; }
@@ -381,11 +370,9 @@ extern "C" int gmsm_fr_poly_fold_device(int fr_field, const void* const* d_polys
     memcpy(g.l, gamma, sizeof(F));
     if (!host_is_reduced(g)) return set_err(GMSM_EINVAL, "gamma is not a reduced fr.Element");
     std::vector<uint64_t> len(lens, lens + k);
-    const unsigned blocks = (unsigned)std::min<uint64_t>((out_len + 255) / 256, GMSM_NUM_SMS * 32u);
-    cudaStream_t st = (cudaStream_t)stream;
-    poly_fold_schedule<P>(reinterpret_cast<const F* const*>(d_polys), len.data(), k, g, [&](const PolyFoldBatch<P>& b, int accumulate) {
-      k_poly_fold<P><<<blocks, 256, 0, st>>>(reinterpret_cast<F*>(d_out), out_len, b, accumulate);
-    });
+    const auto launch = poly_fold_launcher<P>(d_out, out_len, stream);
+    poly_fold_schedule<P>(reinterpret_cast<const F* const*>(d_polys), len.data(), k, g,
+                          [&](const PolyFoldBatch<P>& b, int accumulate) { launch(b, accumulate, false); });
     CK(cudaGetLastError());
     return GMSM_OK;
   });

@@ -43,50 +43,18 @@ extern "C" const char* gmsm_last_error(void) { return g_err.c_str(); }
 extern "C" int gmsm_last_oneshot_launches(void) { return g_last_oneshot_launches; }
 extern "C" const char* gmsm_version(void) { return "gmsm-b200 0.1 (sm_90a)"; }
 
-// ------------------------------------------------------------------------------------------
-// per-curve dispatch
-// ------------------------------------------------------------------------------------------
-static bool curve_info(int curve, CurveInfo* ci) {
-  switch (curve) {
-    case GMSM_BN254_G1: *ci = {bn254_g1::F::N, bn254_fr::BITS, 4 * bn254_fr::N}; return true;
-    case GMSM_BN254_G2: *ci = {bn254_g2::F::N, bn254_fr::BITS, 4 * bn254_fr::N}; return true;
-    case GMSM_BLS12381_G1: *ci = {bls12381_g1::F::N, bls12381_fr::BITS, 4 * bls12381_fr::N}; return true;
-    case GMSM_BLS12381_G2: *ci = {bls12381_g2::F::N, bls12381_fr::BITS, 4 * bls12381_fr::N}; return true;
-    case GMSM_BLS12377_G1: *ci = {bls12377_g1::F::N, bls12377_fr::BITS, 4 * bls12377_fr::N}; return true;
-    case GMSM_BLS12377_G2: *ci = {bls12377_g2::F::N, bls12377_fr::BITS, 4 * bls12377_fr::N}; return true;
-    case GMSM_SECP256K1_G1: *ci = {secp256k1_g1::F::N, secp256k1_fr::BITS, 4 * secp256k1_fr::N}; return true;
-    case GMSM_BW6761_G1: *ci = {bw6761_g1::F::N, bw6761_fr::BITS, 4 * bw6761_fr::N}; return true;
-    case GMSM_BW6761_G2: *ci = {bw6761_g2::F::N, bw6761_fr::BITS, 4 * bw6761_fr::N}; return true;
-    case GMSM_BLS24315_G1: *ci = {bls24315_g1::F::N, bls24315_fr::BITS, 4 * bls24315_fr::N}; return true;
-    case GMSM_BLS24317_G1: *ci = {bls24317_g1::F::N, bls24317_fr::BITS, 4 * bls24317_fr::N}; return true;
-    case GMSM_BW6633_G1: *ci = {bw6633_g1::F::N, bw6633_fr::BITS, 4 * bw6633_fr::N}; return true;
-    case GMSM_BW6633_G2: *ci = {bw6633_g2::F::N, bw6633_fr::BITS, 4 * bw6633_fr::N}; return true;
-  }
-  return false;
+int gmsm::use_device(int device, const char* range_fmt) {
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0) return set_err(GMSM_ENODEV, "no CUDA device (%s); this engine has no CPU fallback", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return set_err(GMSM_EINVAL, range_fmt, device, ndev);
+  if (cudaSetDevice(device) != cudaSuccess) return set_err(GMSM_ECUDA, "cudaSetDevice(%d) failed", device);
+  return GMSM_OK;
 }
 
-extern "C" size_t gmsm_affine_bytes(gmsm_curve_t c) { CurveInfo ci; return curve_info(c, &ci) ? 8u * ci.coord_words : 0; }
-extern "C" size_t gmsm_scalar_bytes(gmsm_curve_t c) { CurveInfo ci; return curve_info(c, &ci) ? (size_t)ci.scalar_bytes : 0; }
-extern "C" size_t gmsm_jac_bytes(gmsm_curve_t c) { CurveInfo ci; return curve_info(c, &ci) ? 12u * ci.coord_words : 0; }
-extern "C" size_t gmsm_xyzz_bytes(gmsm_curve_t c) { CurveInfo ci; return curve_info(c, &ci) ? 16u * ci.coord_words : 0; }
-
-static const GroupVTable* vtable(int curve) {
-  switch (curve) {
-    case GMSM_BN254_G1: return &vt_bn254_g1;
-    case GMSM_BN254_G2: return &vt_bn254_g2;
-    case GMSM_BLS12381_G1: return &vt_bls12381_g1;
-    case GMSM_BLS12381_G2: return &vt_bls12381_g2;
-    case GMSM_BLS12377_G1: return &vt_bls12377_g1;
-    case GMSM_BLS12377_G2: return &vt_bls12377_g2;
-    case GMSM_SECP256K1_G1: return &vt_secp256k1_g1;
-    case GMSM_BW6761_G1: return &vt_bw6761_g1;
-    case GMSM_BW6761_G2: return &vt_bw6761_g2;
-    case GMSM_BLS24315_G1: return &vt_bls24315_g1;
-    case GMSM_BLS24317_G1: return &vt_bls24317_g1;
-    case GMSM_BW6633_G1: return &vt_bw6633_g1;
-    case GMSM_BW6633_G2: return &vt_bw6633_g2;
-  }
-  return nullptr;
+int gmsm::default_device() {
+  const char* e = getenv("GMSM_DEVICE");
+  return e ? atoi(e) : 0;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -112,32 +80,48 @@ struct WidthModel {
   double fixed_ms;        // beyond c = 19: tail = fixed_ms + red19_ms * 2^(c - 19) (the bucket reduction doubles per bit, the carry
   double red19_ms;        //   join / Horner / inversion do not; measured at c = 20, 21); red19_ms = 0: tail_ms[6] * 2^(c - 19)
 };
-static const WidthModel& width_model(int curve) {
-  static const WidthModel bn254_g1 = {0.157, {2.56, 2.43, 2.19, 2.24, 2.41, 3.74, 6.30}, 1.7, 3.0};
-  static const WidthModel bls_g1 = {0.366, {5.29, 5.33, 4.42, 4.59, 5.75, 6.88, 8.53}, 2.85, 4.5};
-  static const WidthModel bn254_g2 = {0.509, {6.50, 6.37, 5.81, 5.95, 5.70, 9.30, 12.0}, 4.45, 6.67};
-  static const WidthModel bls_g2 = {1.300, {13.6, 13.3, 12.2, 12.5, 12.0, 19.6, 25.2}, 0, 0};
-  // N4 remainder: fitted from width sweeps.  secp256k1: fr.Bits = 256 makes the last window narrow for most widths (K1
-  // contention, below).  bw6-761: the 377 doublings of the 24-limb Horner chain dominate its tail.
-  static const WidthModel secp256k1_g1 = {0.1755, {2.50, 2.50, 2.95, 3.08, 3.45, 4.17, 5.66}, 2.05, 3.30};
-  static const WidthModel bw6761 = {1.63, {16.8, 16.5, 17.7, 19.3, 25.9, 30.2, 46.6}, 13.2, 33.4};
-  // 10- and 20-limb groups (bls24-315 / bls24-317 G1, bw6-633): fitted from width sweeps; bw6-633's
-  // c = 17 entry absorbs an accumulate that is slower per addition at that width than at 16 or 18
-  static const WidthModel bls24_g1 = {0.255, {3.38, 3.30, 3.31, 3.50, 3.61, 4.95, 6.18}, 2.5, 3.62};
-  static const WidthModel bw6633 = {1.08, {13.05, 13.3, 12.4, 13.4, 19.6, 18.9, 28.2}, 9.5, 18.7};
-  switch (curve) {
-    case GMSM_SECP256K1_G1: return secp256k1_g1;
-    case GMSM_BW6761_G1: case GMSM_BW6761_G2: return bw6761;
-    case GMSM_BLS24315_G1: case GMSM_BLS24317_G1: return bls24_g1;
-    case GMSM_BW6633_G1: case GMSM_BW6633_G2: return bw6633;
-    case GMSM_BN254_G1: return bn254_g1;
-    case GMSM_BLS12381_G1: case GMSM_BLS12377_G1: return bls_g1;
-    case GMSM_BN254_G2: return bn254_g2;
-    default: return bls_g2;
-  }
-}
+static const WidthModel WM_BN254_G1 = {0.157, {2.56, 2.43, 2.19, 2.24, 2.41, 3.74, 6.30}, 1.7, 3.0};
+static const WidthModel WM_BLS_G1 = {0.366, {5.29, 5.33, 4.42, 4.59, 5.75, 6.88, 8.53}, 2.85, 4.5};
+static const WidthModel WM_BN254_G2 = {0.509, {6.50, 6.37, 5.81, 5.95, 5.70, 9.30, 12.0}, 4.45, 6.67};
+static const WidthModel WM_BLS_G2 = {1.300, {13.6, 13.3, 12.2, 12.5, 12.0, 19.6, 25.2}, 0, 0};
+// N4 remainder: fitted from width sweeps.  secp256k1: fr.Bits = 256 makes the last window narrow for most widths (K1
+// contention, below).  bw6-761: the 377 doublings of the 24-limb Horner chain dominate its tail.
+static const WidthModel WM_SECP256K1_G1 = {0.1755, {2.50, 2.50, 2.95, 3.08, 3.45, 4.17, 5.66}, 2.05, 3.30};
+static const WidthModel WM_BW6761 = {1.63, {16.8, 16.5, 17.7, 19.3, 25.9, 30.2, 46.6}, 13.2, 33.4};
+// 10- and 20-limb groups (bls24-315 / bls24-317 G1, bw6-633): fitted from width sweeps; bw6-633's
+// c = 17 entry absorbs an accumulate that is slower per addition at that width than at 16 or 18
+static const WidthModel WM_BLS24_G1 = {0.255, {3.38, 3.30, 3.31, 3.50, 3.61, 4.95, 6.18}, 2.5, 3.62};
+static const WidthModel WM_BW6633 = {1.08, {13.05, 13.3, 12.4, 13.4, 19.6, 18.9, 28.2}, 9.5, 18.7};
+
+// per-group dispatch: one row per gmsm_curve_t, in the order of its ids
+struct Group {
+  const GroupVTable* vt;   // kernels and type sizes (inst_*.cu)
+  int fr_field;            // GMSM_FR_* of kzg.ToLagrangeG1, -1 for the groups without it
+  const WidthModel* wm;
+};
+// The vtables are defined in other translation units: this table holds their addresses only, and nothing reads them
+// before main() starts.
+static const Group GROUPS[] = {
+    {&vt_bn254_g1, GMSM_FR_BN254, &WM_BN254_G1},          {&vt_bn254_g2, -1, &WM_BN254_G2},
+    {&vt_bls12381_g1, GMSM_FR_BLS12381, &WM_BLS_G1},      {&vt_bls12381_g2, -1, &WM_BLS_G2},
+    {&vt_bls12377_g1, GMSM_FR_BLS12377, &WM_BLS_G1},      {&vt_bls12377_g2, -1, &WM_BLS_G2},
+    {&vt_secp256k1_g1, -1, &WM_SECP256K1_G1},
+    {&vt_bw6761_g1, GMSM_FR_BW6761, &WM_BW6761},          {&vt_bw6761_g2, -1, &WM_BW6761},
+    {&vt_bls24315_g1, GMSM_FR_BLS24315, &WM_BLS24_G1},    {&vt_bls24317_g1, GMSM_FR_BLS24317, &WM_BLS24_G1},
+    {&vt_bw6633_g1, GMSM_FR_BW6633, &WM_BW6633},          {&vt_bw6633_g2, -1, &WM_BW6633},
+};
+static_assert(sizeof(GROUPS) / sizeof(GROUPS[0]) == GMSM_BW6633_G2 + 1, "one row per gmsm_curve_t");
+
+static const Group* group(int curve) { return curve >= 0 && curve <= GMSM_BW6633_G2 ? &GROUPS[curve] : nullptr; }
+static const GroupVTable* vtable(int curve) { return group(curve) ? group(curve)->vt : nullptr; }
+
+extern "C" size_t gmsm_affine_bytes(gmsm_curve_t c) { const GroupVTable* vt = vtable(c); return vt ? 8u * vt->ci.coord_words : 0; }
+extern "C" size_t gmsm_scalar_bytes(gmsm_curve_t c) { const GroupVTable* vt = vtable(c); return vt ? (size_t)vt->ci.scalar_bytes : 0; }
+extern "C" size_t gmsm_jac_bytes(gmsm_curve_t c) { const GroupVTable* vt = vtable(c); return vt ? 12u * vt->ci.coord_words : 0; }
+extern "C" size_t gmsm_xyzz_bytes(gmsm_curve_t c) { const GroupVTable* vt = vtable(c); return vt ? 16u * vt->ci.coord_words : 0; }
+
 static double model_ms(int curve, int fr_bits, size_t n, int c) {
-  const WidthModel& m = width_model(curve);
+  const WidthModel& m = *group(curve)->wm;
   const WindowPlan p = make_plan(fr_bits, c);
   double tail;
   if (c < 13) tail = m.tail_ms[0] * (1.0 + 0.03 * (13 - c));        // more windows: longer Horner / more launches, fewer buckets
@@ -165,10 +149,6 @@ static int choose_c_for(int curve, int fr_bits, size_t n) {
   }
   return bc;
 }
-static int curve_of_bits_default(int fr_bits) {
-  return fr_bits == 254 ? GMSM_BN254_G1 : fr_bits == 255 ? GMSM_BLS12381_G1 : fr_bits == 256 ? GMSM_SECP256K1_G1 : fr_bits == 377 ? GMSM_BW6761_G1 : fr_bits == 315 ? GMSM_BW6633_G1 : GMSM_BLS12377_G1;
-}
-static int choose_c(int fr_bits, size_t n) { return choose_c_for(curve_of_bits_default(fr_bits), fr_bits, n); }
 
 // window width of the window-table mode: one shared bucket set, so the bucket reduction costs 2^(c-1) * ~3.8
 // full-add equivalents ONCE instead of per window, and c can grow until that term meets the W(c)*n accumulate
@@ -316,14 +296,11 @@ extern "C" gmsm_ctx_t* gmsm_ctx_create_tables(gmsm_curve_t curve, size_t max_n, 
 }
 
 static gmsm_ctx* ctx_create_ex(gmsm_curve_t curve, size_t max_n, int c, int device, bool shared) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) { set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve); return nullptr; }
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) { set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve); return nullptr; }
   if (c != 0 && (c < 2 || c > 24)) { set_err(GMSM_EINVAL, "window width c=%d out of range [2,24]", c); return nullptr; }
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) { set_err(GMSM_ENODEV, "no CUDA device (%s); this engine has no CPU fallback", cudaGetErrorString(e)); return nullptr; }
-  if (device < 0 || device >= ndev) { set_err(GMSM_EINVAL, "device %d out of range (%d devices)", device, ndev); return nullptr; }
-  if (cudaSetDevice(device) != cudaSuccess) { set_err(GMSM_ECUDA, "cudaSetDevice(%d) failed", device); return nullptr; }
+  if (use_device(device) != GMSM_OK) return nullptr;
+  const CurveInfo& ci = vt->ci;
   if (max_n == 0) max_n = 1;
   l2_granularity_acquire(device);
   gmsm_ctx* ctx = new gmsm_ctx();
@@ -412,6 +389,14 @@ struct CtxCall {
   ~CtxCall() { cudaEventRecord(c->ev_done, st); }
 };
 
+// the last two stage events of a profiled call (gmsm_ctx_last_stage_ms)
+static void record_stage_end(gmsm_ctx* ctx, cudaStream_t st) {
+  if (!ctx->profiling) return;
+  cudaEventRecord(ctx->ev[7], st);
+  cudaEventRecord(ctx->ev[8], st);
+  ctx->have_stage = true;
+}
+
 extern "C" int gmsm_ctx_window_sums_device(gmsm_ctx_t* ctx, const void* d_points, const void* d_scalars, size_t n,
                                            void* d_partials, void* stream) {
   if (!ctx) return set_err(GMSM_EINVAL, "null ctx");
@@ -419,13 +404,8 @@ extern "C" int gmsm_ctx_window_sums_device(gmsm_ctx_t* ctx, const void* d_points
   if (n > ctx->max_n) return set_err(GMSM_EINVAL, "n=%zu exceeds ctx capacity %zu", n, ctx->max_n);
   CtxCall call(ctx, (cudaStream_t)stream);
   if (int rc0 = call.begin()) return rc0;
-  int rc = GMSM_OK;
-  rc = vtable(ctx->curve)->window_sums(ctx, d_points, d_scalars, n, d_partials, (cudaStream_t)stream);
-  if (rc == GMSM_OK && ctx->profiling) {
-    cudaEventRecord(ctx->ev[7], (cudaStream_t)stream);
-    cudaEventRecord(ctx->ev[8], (cudaStream_t)stream);
-    ctx->have_stage = true;
-  }
+  const int rc = vtable(ctx->curve)->window_sums(ctx, d_points, d_scalars, n, d_partials, (cudaStream_t)stream);
+  if (rc == GMSM_OK) record_stage_end(ctx, (cudaStream_t)stream);
   return rc;
 }
 
@@ -440,26 +420,27 @@ extern "C" int gmsm_ctx_finalize_device(gmsm_ctx_t* ctx, const void* d_partials,
   return rc;
 }
 
+// one whole MSM on the context: window sums, then finalize.  tab_stride: points per table row of a window-table context
+static int ctx_msm(gmsm_ctx* ctx, const void* d_points, size_t tab_stride, const void* d_scalars, size_t n, void* d_out_jac,
+                   void* stream) {
+  CtxCall call(ctx, (cudaStream_t)stream);
+  if (int rc0 = call.begin()) return rc0;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (ctx->shared) ctx->tab_stride = (uint32_t)tab_stride;
+  const GroupVTable* vt = vtable(ctx->curve);
+  if (int rc = vt->window_sums(ctx, d_points, d_scalars, n, ctx->win_partials, st)) return rc;
+  if (int rc = vt->finalize(ctx, ctx->win_partials, 1, d_out_jac, st)) return rc;
+  ctx->last_launches += 1;
+  record_stage_end(ctx, st);
+  return GMSM_OK;
+}
+
 extern "C" int gmsm_ctx_msm_device(gmsm_ctx_t* ctx, const void* d_points, const void* d_scalars, size_t n,
                                    void* d_out_jac, void* stream) {
   if (!ctx) return set_err(GMSM_EINVAL, "null ctx");
   if (ctx->shared) return set_err(GMSM_EINVAL, "window-table context: use gmsm_ctx_msm_tables_device");
   if (n > ctx->max_n) return set_err(GMSM_EINVAL, "n=%zu exceeds ctx capacity %zu", n, ctx->max_n);
-  CtxCall call(ctx, (cudaStream_t)stream);
-  if (int rc0 = call.begin()) return rc0;
-  int rc = GMSM_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  rc = vtable(ctx->curve)->window_sums(ctx, d_points, d_scalars, n, ctx->win_partials, st);
-  if (rc != GMSM_OK) return rc;
-  rc = vtable(ctx->curve)->finalize(ctx, ctx->win_partials, 1, d_out_jac, st);
-  if (rc != GMSM_OK) return rc;
-  ctx->last_launches += 1;
-  if (ctx->profiling) {
-    cudaEventRecord(ctx->ev[7], st);
-    cudaEventRecord(ctx->ev[8], st);
-    ctx->have_stage = true;
-  }
-  return GMSM_OK;
+  return ctx_msm(ctx, d_points, 0, d_scalars, n, d_out_jac, stream);
 }
 
 // make the device that owns a device pointer current (entry points that take raw device pointers and no context:
@@ -477,21 +458,21 @@ static int set_device_of(const void* dptr) {
 // ---- window tables (device level) ----
 extern "C" int gmsm_tables_build_device(gmsm_curve_t curve, int c, const void* d_points, size_t n, void* d_table,
                                         size_t row_stride, void* stream) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
   if (c < 2 || c > 24) return set_err(GMSM_EINVAL, "window width c=%d out of range [2,24]", c);
   if (row_stride < n) return set_err(GMSM_EINVAL, "row_stride %zu < n %zu", row_stride, n);
-  const WindowPlan p = make_plan(ci.fr_bits, c);
+  const WindowPlan p = make_plan(vt->ci.fr_bits, c);
   if ((double)row_stride * p.nwin >= 2147483000.0)
     return set_err(GMSM_EINVAL, "row_stride*W = %zu*%d does not fit the 31-bit table index; shard the bases", row_stride, p.nwin);
   if (n == 0) return GMSM_OK;
   if (int rc = set_device_of(d_table)) return rc;
-  const size_t ab = 8u * ci.coord_words;
+  const size_t ab = 8u * vt->ci.coord_words;
   cudaStream_t st = (cudaStream_t)stream;
   if (d_table != d_points) CK(cudaMemcpyAsync(d_table, d_points, n * ab, cudaMemcpyDeviceToDevice, st));
   for (int j = 1; j < p.nwin; j++) {
-    if (int rc = vtable(curve)->table_level((const char*)d_table + (size_t)(j - 1) * row_stride * ab, n, c,
-                                            (char*)d_table + (size_t)j * row_stride * ab, st)) return rc;
+    if (int rc = vt->table_level((const char*)d_table + (size_t)(j - 1) * row_stride * ab, n, c,
+                                 (char*)d_table + (size_t)j * row_stride * ab, st)) return rc;
   }
   return GMSM_OK;
 }
@@ -503,22 +484,8 @@ extern "C" int gmsm_ctx_msm_tables_device(gmsm_ctx_t* ctx, const void* d_table, 
   if (n > ctx->max_n) return set_err(GMSM_EINVAL, "n=%zu exceeds ctx capacity %zu", n, ctx->max_n);
   if (offset > row_stride || n > row_stride - offset) return set_err(GMSM_EINVAL, "len(points) != len(scalars)");
   if ((double)row_stride * ctx->plan.nwin >= 2147483000.0) return set_err(GMSM_EINVAL, "row_stride*W does not fit the 31-bit table index");
-  CtxCall call(ctx, (cudaStream_t)stream);
-  if (int rc0 = call.begin()) return rc0;
-  cudaStream_t st = (cudaStream_t)stream;
-  ctx->tab_stride = (uint32_t)row_stride;
   const size_t ab = 8u * ctx->ci.coord_words;
-  int rc = vtable(ctx->curve)->window_sums(ctx, (const char*)d_table + offset * ab, d_scalars, n, ctx->win_partials, st);
-  if (rc != GMSM_OK) return rc;
-  rc = vtable(ctx->curve)->finalize(ctx, ctx->win_partials, 1, d_out_jac, st);
-  if (rc != GMSM_OK) return rc;
-  ctx->last_launches += 1;
-  if (ctx->profiling) {
-    cudaEventRecord(ctx->ev[7], st);
-    cudaEventRecord(ctx->ev[8], st);
-    ctx->have_stage = true;
-  }
-  return GMSM_OK;
+  return ctx_msm(ctx, (const char*)d_table + offset * ab, row_stride, d_scalars, n, d_out_jac, stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -560,7 +527,6 @@ class CopyPool {
     std::unique_lock<std::mutex> lk(job.mu);
     job.cv.wait(lk, [&] { return job.remaining.load() == 0; });
   }
-  int threads() const { return nthreads_; }
 
  private:
   static constexpr size_t PART = 2 << 20;
@@ -676,8 +642,12 @@ struct Pipeline {
   size_t tab_stride = 0;
   int tab_c = 0;
   Stager stager;          // pinned ring for pageable caller buffers
-  int last_staged = 0;    // 1 if the last call went through the ring
+  void* d_gather = nullptr;   // the window partials of all shards of a sharded call that this pipeline joins
+  size_t gather_cap = 0;
 };
+
+// the rule of every grow-only buffer kept between calls: rebuilt when smaller than n or more than 4x oversized
+static bool needs_resize(size_t cap, size_t n) { return cap < n || cap > 4 * n + 1024; }
 
 static int pipeline_init(Pipeline& P, int curve, int device) {
   if (P.copy_st) return GMSM_OK;
@@ -692,11 +662,21 @@ static int pipeline_init(Pipeline& P, int curve, int device) {
 static void pipeline_free(Pipeline& P) {
   if (P.ctx) gmsm_ctx_destroy(P.ctx);
   P.stager.release();
-  cudaFree(P.d_scalars); cudaFree(P.d_partials); cudaFree(P.d_out);
+  cudaFree(P.d_scalars); cudaFree(P.d_partials); cudaFree(P.d_out); cudaFree(P.d_gather);
   if (P.copy_st) cudaStreamDestroy(P.copy_st);
   if (P.comp_st) cudaStreamDestroy(P.comp_st);
   for (int i = 0; i < 16; i++) if (P.ev[i]) cudaEventDestroy(P.ev[i]);
   P = Pipeline();
+}
+
+// P.ctx for n points at width c, rebuilt unless the one kept from earlier calls fits: its capacity (needs_resize), width,
+// table mode and the GMSM_* knobs it was built under
+static int pipeline_ctx(Pipeline& P, size_t n, int c) {
+  if (P.ctx && !needs_resize(P.ctx->max_n, n) && P.ctx->plan.c == c && P.ctx->shared == P.tables && P.ctx->knobs == knob_signature())
+    return GMSM_OK;
+  if (P.ctx) { gmsm_ctx_destroy(P.ctx); P.ctx = nullptr; }
+  P.ctx = ctx_create_ex((gmsm_curve_t)P.curve, n, c, P.device, P.tables);
+  return P.ctx ? GMSM_OK : GMSM_ECUDA;
 }
 
 // d_points: device buffer holding (resident) or receiving (h_points != nullptr) the n points
@@ -705,8 +685,8 @@ static void pipeline_free(Pipeline& P) {
 // (host copy) instead of the finalized point.
 static int pipeline_run(Pipeline& P, void* d_points, const uint64_t* h_points, const uint64_t* h_scalars, size_t n,
                         uint64_t* out_jac, int c_force = 0, void* h_partials = nullptr) {
-  CurveInfo ci;
-  curve_info(P.curve, &ci);
+  const GroupVTable* vt = vtable(P.curve);
+  const CurveInfo& ci = vt->ci;
   const size_t sb = (size_t)ci.scalar_bytes;
   const size_t ab = 8u * ci.coord_words, xb = 16u * ci.coord_words, jb = 12u * ci.coord_words;
   CK(cudaSetDevice(P.device));
@@ -747,19 +727,14 @@ static int pipeline_run(Pipeline& P, void* d_points, const uint64_t* h_points, c
   }
   size_t nc = 0;
   for (int k = 0; k < nch; k++) nc = std::max(nc, bstart[k + 1] - bstart[k]);
-  if (P.scal_cap < n || P.scal_cap > 4 * n + 1024) {
+  if (needs_resize(P.scal_cap, n)) {
     cudaFree(P.d_scalars); P.d_scalars = nullptr; P.scal_cap = 0;
     CK(cudaMalloc(&P.d_scalars, n * (size_t)ci.scalar_bytes));
     P.scal_cap = n;
   }
   // window width from the TOTAL size (all batches share one bucket array); workspace sized for one batch
   const int c = P.tables ? P.tab_c : (c_force ? c_force : choose_c_for(P.curve, ci.fr_bits, n));
-  if (!P.ctx || P.ctx->max_n < nc || P.ctx->max_n > 4 * nc + 1024 || P.ctx->plan.c != c || P.ctx->shared != P.tables ||
-      P.ctx->knobs != knob_signature()) {
-    if (P.ctx) { gmsm_ctx_destroy(P.ctx); P.ctx = nullptr; }
-    P.ctx = ctx_create_ex((gmsm_curve_t)P.curve, nc, c, P.device, P.tables);
-    if (!P.ctx) return GMSM_ECUDA;
-  }
+  if (int rc = pipeline_ctx(P, nc, c)) return rc;
   P.ctx->tab_stride = (uint32_t)P.tab_stride;
   const int npart = P.ctx->red_windows();   // partials per batch / per call: W, or 1 in window-table mode
   if (P.partials_cap < nch * npart) {
@@ -767,7 +742,6 @@ static int pipeline_run(Pipeline& P, void* d_points, const uint64_t* h_points, c
     CK(cudaMalloc(&P.d_partials, (size_t)nch * npart * xb));
     P.partials_cap = nch * npart;
   }
-  const GroupVTable* vt = vtable(P.curve);
   const char* hp = reinterpret_cast<const char*>(h_points);
   const char* hs = reinterpret_cast<const char*>(h_scalars);
   // the batch-affine path keeps per-batch partials instead (and cannot return per-device partials)
@@ -794,7 +768,6 @@ static int pipeline_run(Pipeline& P, void* d_points, const uint64_t* h_points, c
   if (const char* e = getenv("GMSM_STAGING")) staging = atoi(e) != 0;
   const bool stage_scalars = staging && n * (size_t)ci.scalar_bytes >= (1u << 20) && !host_pointer_is_pinned(hs);
   const bool stage_points = staging && hp && n * ab >= (1u << 20) && !host_pointer_is_pinned(hp);
-  P.last_staged = (stage_scalars || stage_points) ? 1 : 0;
   auto h2d = [&](void* dst, const char* src, size_t bytes, bool staged) -> int {
     if (staged) return P.stager.copy(dst, src, bytes, P.copy_st);
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, P.copy_st));
@@ -841,40 +814,65 @@ static int pipeline_run(Pipeline& P, void* d_points, const uint64_t* h_points, c
   return GMSM_OK;
 }
 
-static int check_device(int device) {
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) return set_err(GMSM_ENODEV, "no CUDA device (%s); this engine has no CPU fallback", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return set_err(GMSM_EINVAL, "device %d out of range (%d devices)", device, ndev);
-  return GMSM_OK;
-}
-
 static int check_nb_tasks(int nb_tasks) {
   // (*G1Jac).MultiExp, multiexp.go:67-71
   if (nb_tasks > 1024) return set_err(GMSM_EINVAL, "invalid config: config.NbTasks > 1024");
   return GMSM_OK;
 }
 
-// join the W window partials of D shards (host copy, shard-major) on the device of pipeline P0:
+// join the window partials of D shards (host copy, shard-major) on the device of pipeline P0:
 // per-window sum over the shards, Horner, normalisation -> out_jac (host)
-static int join_partials(int curve, Pipeline& P0, void** d_gather, size_t* gather_cap, const unsigned char* h_part,
-                         size_t bytes, int D, uint64_t* out_jac) {
-  CurveInfo ci;
-  curve_info(curve, &ci);
+static int join_partials(Pipeline& P0, const unsigned char* h_part, size_t bytes, int D, uint64_t* out_jac) {
+  const GroupVTable* vt = vtable(P0.curve);
   CK(cudaSetDevice(P0.device));
-  if (*gather_cap < bytes) {
-    cudaFree(*d_gather); *d_gather = nullptr;
-    CK(cudaMalloc(d_gather, bytes));
-    *gather_cap = bytes;
+  if (P0.gather_cap < bytes) {
+    cudaFree(P0.d_gather); P0.d_gather = nullptr;
+    CK(cudaMalloc(&P0.d_gather, bytes));
+    P0.gather_cap = bytes;
   }
-  CK(cudaMemcpyAsync(*d_gather, h_part, bytes, cudaMemcpyHostToDevice, P0.comp_st));
+  CK(cudaMemcpyAsync(P0.d_gather, h_part, bytes, cudaMemcpyHostToDevice, P0.comp_st));
   {
     std::lock_guard<std::mutex> lk2(P0.ctx->mu);
-    if (int rc = vtable(curve)->finalize(P0.ctx, *d_gather, D, P0.d_out, P0.comp_st)) return rc;
+    if (int rc = vt->finalize(P0.ctx, P0.d_gather, D, P0.d_out, P0.comp_st)) return rc;
   }
-  CK(cudaMemcpyAsync(out_jac, P0.d_out, 12u * ci.coord_words, cudaMemcpyDeviceToHost, P0.comp_st));
+  CK(cudaMemcpyAsync(out_jac, P0.d_out, 12u * vt->ci.coord_words, cudaMemcpyDeviceToHost, P0.comp_st));
   CK(cudaStreamSynchronize(P0.comp_st));
   return GMSM_OK;
+}
+
+// one shard of a sharded call: n points on the device of `pipe`, resident there or copied from h_points
+struct Shard {
+  Pipeline* pipe;
+  void* d_points;
+  const uint64_t* h_points;
+  const uint64_t* h_scalars;
+  size_t n;
+};
+
+// runs every shard's pipeline on a host thread of its own, all at window width c, and joins their partials on the first
+// shard's pipeline.  In window-table mode each shard returns ONE partial.
+static int run_shards(const std::vector<Shard>& shards, int c, uint64_t* out_jac) {
+  Pipeline& P0 = *shards[0].pipe;
+  const CurveInfo& ci = vtable(P0.curve)->ci;
+  const size_t npart = P0.tables ? 1 : (size_t)make_plan(ci.fr_bits, c).nwin;
+  const size_t part_bytes = npart * 16u * ci.coord_words;
+  std::vector<unsigned char> h_part(shards.size() * part_bytes);
+  std::vector<int> rcs(shards.size(), GMSM_OK);
+  std::vector<std::string> errs(shards.size());
+  {
+    std::vector<std::thread> th;
+    for (size_t k = 0; k < shards.size(); k++) {
+      th.emplace_back([&, k]() {
+        const Shard& s = shards[k];
+        rcs[k] = pipeline_run(*s.pipe, s.d_points, s.h_points, s.h_scalars, s.n, nullptr, c, h_part.data() + k * part_bytes);
+        if (rcs[k]) errs[k] = g_err;   // thread-local error text of the worker
+      });
+    }
+    for (auto& t : th) t.join();
+  }
+  for (size_t k = 0; k < shards.size(); k++)
+    if (rcs[k]) return set_err(rcs[k], "device %d: %s", shards[k].pipe->device, errs[k].c_str());
+  return join_partials(P0, h_part.data(), h_part.size(), (int)shards.size(), out_jac);
 }
 
 // the devices listed in GMSM_DEVICES ("0,1,2,3"), empty if unset
@@ -900,8 +898,6 @@ struct BaseShard {
   size_t lo = 0, hi = 0;
   void* d_points = nullptr;
   Pipeline pipe;
-  void* d_gather = nullptr;
-  size_t gather_cap = 0;
 };
 struct gmsm_bases {
   int curve = 0;
@@ -913,8 +909,8 @@ struct gmsm_bases {
 extern "C" void gmsm_bases_free(gmsm_bases_t* b);
 
 extern "C" gmsm_bases_t* gmsm_bases_upload(gmsm_curve_t curve, const uint64_t* points, size_t n, int device) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) { set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve); return nullptr; }
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) { set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve); return nullptr; }
   std::vector<int> devs;
   if (device == -1) {
     devs = env_devices();
@@ -922,8 +918,8 @@ extern "C" gmsm_bases_t* gmsm_bases_upload(gmsm_curve_t curve, const uint64_t* p
   } else {
     devs.push_back(device);
   }
-  for (int d : devs) if (check_device(d) != GMSM_OK) return nullptr;
-  const size_t ab = 8u * ci.coord_words;
+  for (int d : devs) if (use_device(d) != GMSM_OK) return nullptr;
+  const size_t ab = 8u * vt->ci.coord_words;
   gmsm_bases* b = new gmsm_bases();
   b->curve = curve; b->n = n;
   b->shards.resize(devs.size());
@@ -953,8 +949,7 @@ extern "C" int gmsm_bases_precompute(gmsm_bases_t* b, int c) {
   if (!b) return set_err(GMSM_EINVAL, "null bases");
   if (c != 0 && (c < 2 || c > 24)) return set_err(GMSM_EINVAL, "window width c=%d out of range [2,24]", c);
   std::lock_guard<std::mutex> lk(b->mu);
-  CurveInfo ci;
-  curve_info(b->curve, &ci);
+  const CurveInfo& ci = vtable(b->curve)->ci;
   const size_t ab = 8u * ci.coord_words;
   size_t max_sh = 0;
   for (BaseShard& sh : b->shards) {
@@ -1014,7 +1009,6 @@ extern "C" void gmsm_bases_free(gmsm_bases_t* b) {
     cudaSetDevice(sh.device);
     pipeline_free(sh.pipe);
     cudaFree(sh.d_points);
-    cudaFree(sh.d_gather);
   }
   delete b;
 }
@@ -1025,47 +1019,24 @@ extern "C" int gmsm_bases_multiexp(gmsm_bases_t* b, size_t offset, const uint64_
   if (int rc = check_nb_tasks(nb_tasks)) return rc;
   if (offset > b->n || n > b->n - offset) return set_err(GMSM_EINVAL, "len(points) != len(scalars)");
   std::lock_guard<std::mutex> lk(b->mu);
-  CurveInfo ci;
-  curve_info(b->curve, &ci);
-  const size_t ab = 8u * ci.coord_words, xb = 16u * ci.coord_words;
+  const CurveInfo& ci = vtable(b->curve)->ci;
+  const size_t ab = 8u * ci.coord_words;
   if (n == 0) { memset(out_jac, 0, 12u * ci.coord_words); return GMSM_OK; }
   // shards intersecting [offset, offset + n)
-  struct Job { BaseShard* sh; size_t a, e; };
-  std::vector<Job> jobs;
+  std::vector<Shard> shards;
+  size_t largest = 0;
   for (BaseShard& sh : b->shards) {
     const size_t a = std::max(sh.lo, offset), e = std::min(sh.hi, offset + n);
-    if (a < e) jobs.push_back({&sh, a, e});
+    if (a >= e) continue;
+    shards.push_back({&sh.pipe, reinterpret_cast<char*>(sh.d_points) + (a - sh.lo) * ab, nullptr,
+                      scalars + (a - offset) * (size_t)(ci.scalar_bytes / 8), e - a});
+    largest = std::max(largest, e - a);
   }
-  if (jobs.size() == 1) {
-    BaseShard& sh = *jobs[0].sh;
-    return pipeline_run(sh.pipe, reinterpret_cast<char*>(sh.d_points) + (jobs[0].a - sh.lo) * ab, nullptr, scalars, n, out_jac);
-  }
-  // window-table mode: every shard carries the same table width and returns ONE partial
-  const bool tables = jobs[0].sh->pipe.tables;
-  size_t largest = 0;
-  for (const auto& j : jobs) largest = std::max(largest, (size_t)(j.e - j.a));
-  const int c = tables ? jobs[0].sh->pipe.tab_c : choose_c_for(b->curve, ci.fr_bits, largest);   // the plan of the largest shard, on all of them
-  const WindowPlan plan = make_plan(ci.fr_bits, c);
-  const size_t npart = tables ? 1 : (size_t)plan.nwin;
-  std::vector<unsigned char> h_part(jobs.size() * npart * xb);
-  std::vector<int> rcs(jobs.size(), GMSM_OK);
-  std::vector<std::string> errs(jobs.size());
-  {
-    std::vector<std::thread> th;
-    for (size_t k = 0; k < jobs.size(); k++) {
-      th.emplace_back([&, k]() {
-        const Job& j = jobs[k];
-        rcs[k] = pipeline_run(j.sh->pipe, reinterpret_cast<char*>(j.sh->d_points) + (j.a - j.sh->lo) * ab, nullptr,
-                              scalars + (j.a - offset) * (size_t)(ci.scalar_bytes / 8), j.e - j.a, nullptr, c, h_part.data() + k * npart * xb);
-        if (rcs[k]) errs[k] = g_err;
-      });
-    }
-    for (auto& t : th) t.join();
-  }
-  for (size_t k = 0; k < jobs.size(); k++)
-    if (rcs[k]) return set_err(rcs[k], "device %d: %s", jobs[k].sh->device, errs[k].c_str());
-  BaseShard& s0 = *jobs[0].sh;
-  return join_partials(b->curve, s0.pipe, &s0.d_gather, &s0.gather_cap, h_part.data(), h_part.size(), (int)jobs.size(), out_jac);
+  if (shards.size() == 1) return pipeline_run(*shards[0].pipe, shards[0].d_points, nullptr, scalars, n, out_jac);
+  // window-table mode: every shard carries the same table width
+  const Pipeline& P0 = *shards[0].pipe;
+  const int c = P0.tables ? P0.tab_c : choose_c_for(b->curve, ci.fr_bits, largest);   // the plan of the largest shard, on all of them
+  return run_shards(shards, c, out_jac);
 }
 
 // MSM over resident bases with scalars that are ALREADY on the device (the output of a device-side iFFT, gmsm_fft_device:
@@ -1079,20 +1050,14 @@ extern "C" int gmsm_bases_multiexp_device(gmsm_bases_t* b, size_t offset, const 
   if (offset > b->n || n > b->n - offset) return set_err(GMSM_EINVAL, "len(points) != len(scalars)");
   if (b->shards.size() != 1) return set_err(GMSM_EINVAL, "device scalars need bases that live on one device (this handle is sharded over %zu)", b->shards.size());
   std::lock_guard<std::mutex> lk(b->mu);
-  CurveInfo ci;
-  curve_info(b->curve, &ci);
+  const CurveInfo& ci = vtable(b->curve)->ci;
   const size_t ab = 8u * ci.coord_words, jb = 12u * ci.coord_words;
   if (n == 0) { memset(out_jac, 0, jb); return GMSM_OK; }
   BaseShard& sh = b->shards[0];
   Pipeline& P = sh.pipe;
   CK(cudaSetDevice(P.device));
   const int c = P.tables ? P.tab_c : choose_c_for(P.curve, ci.fr_bits, n);
-  if (!P.ctx || P.ctx->max_n < n || P.ctx->max_n > 4 * n + 1024 || P.ctx->plan.c != c || P.ctx->shared != P.tables ||
-      P.ctx->knobs != knob_signature()) {
-    if (P.ctx) { gmsm_ctx_destroy(P.ctx); P.ctx = nullptr; }
-    P.ctx = ctx_create_ex((gmsm_curve_t)P.curve, n, c, P.device, P.tables);
-    if (!P.ctx) return GMSM_ECUDA;
-  }
+  if (int rc = pipeline_ctx(P, n, c)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
   if (P.tables)
@@ -1115,8 +1080,6 @@ struct Session {
   Pipeline pipe;
   void* d_points = nullptr;
   size_t cap = 0;
-  void* d_gather = nullptr;
-  size_t gather_cap = 0;
   bool busy = false;
 };
 static std::mutex g_sess_mu;
@@ -1156,34 +1119,31 @@ struct SessionLease {
 
 // size the leased session's point buffer for cnt points (exclusive access: the lease)
 static int session_prepare(Session& S, int curve, int device, size_t cnt) {
-  CurveInfo ci;
-  curve_info(curve, &ci);
   CK(cudaSetDevice(device));
   if (int rc = pipeline_init(S.pipe, curve, device)) return rc;
-  if (S.cap < cnt || S.cap > 4 * cnt + 1024) {
+  if (needs_resize(S.cap, cnt)) {
     cudaFree(S.d_points); S.d_points = nullptr; S.cap = 0;
-    CK(cudaMalloc(&S.d_points, cnt * 8u * ci.coord_words));
+    CK(cudaMalloc(&S.d_points, cnt * 8u * vtable(curve)->ci.coord_words));
     S.cap = cnt;
   }
   return GMSM_OK;
 }
 
 extern "C" int gmsm_choose_window_bits(gmsm_curve_t curve, size_t n_total) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) return 0;
-  return choose_c_for(curve, ci.fr_bits, n_total);
+  const GroupVTable* vt = vtable(curve);
+  return vt ? choose_c_for(curve, vt->ci.fr_bits, n_total) : 0;
 }
 
 // one shard of a sharded call, host buffers in, W window partials (host) out: the pipelined engine of
 // gmsm_multiexp without the finalize.  All shards must use the same window width c.
 extern "C" int gmsm_multiexp_window_sums(gmsm_curve_t curve, const uint64_t* points, const uint64_t* scalars, size_t n, int c,
                                          int device, void* out_partials) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
   if (c < 2 || c > 24) return set_err(GMSM_EINVAL, "window width c=%d out of range [2,24]", c);
-  if (int rc = check_device(device)) return rc;
-  const WindowPlan plan = make_plan(ci.fr_bits, c);
-  if (n == 0) { memset(out_partials, 0, (size_t)plan.nwin * 16u * ci.coord_words); return GMSM_OK; }
+  if (int rc = use_device(device)) return rc;
+  const WindowPlan plan = make_plan(vt->ci.fr_bits, c);
+  if (n == 0) { memset(out_partials, 0, (size_t)plan.nwin * 16u * vt->ci.coord_words); return GMSM_OK; }
   SessionLease lease;
   lease.acquire(curve, device);
   if (int rc = session_prepare(*lease.S, curve, device, n)) return rc;
@@ -1193,17 +1153,14 @@ extern "C" int gmsm_multiexp_window_sums(gmsm_curve_t curve, const uint64_t* poi
 extern "C" int gmsm_multiexp(gmsm_curve_t curve, const uint64_t* points, const uint64_t* scalars, size_t n, int nb_tasks,
                              uint64_t* out_jac) {
   if (int rc = check_nb_tasks(nb_tasks)) return rc;
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  const CurveInfo& ci = vt->ci;
   // devices: GMSM_DEVICES="0,1,2,3" shards one call over several GPUs of this process (one host thread per
   // device, the per-device window partials joined on the first one); default: the single GMSM_DEVICE (0)
   std::vector<int> devs = env_devices();
-  if (devs.empty()) {
-    int device = 0;
-    if (const char* e = getenv("GMSM_DEVICE")) device = atoi(e);
-    devs.push_back(device);
-  }
-  for (int d : devs) if (int rc = check_device(d)) return rc;
+  if (devs.empty()) devs.push_back(default_device());
+  for (int d : devs) if (int rc = use_device(d)) return rc;
   if (n == 0) { memset(out_jac, 0, 12u * ci.coord_words); return GMSM_OK; }
   const size_t ab = 8u * ci.coord_words;
   const size_t D = (n >= ((size_t)1 << 16)) ? devs.size() : 1;   // small calls stay on one device
@@ -1216,35 +1173,16 @@ extern "C" int gmsm_multiexp(gmsm_curve_t curve, const uint64_t* points, const u
   // ---- multi-device: contiguous shards (the reference's recursive halving, multiexp.go:128-140) ----
   // one plan for every shard (their partials are added window by window), sized for the work ONE device does: the largest shard
   const int c = choose_c_for(curve, ci.fr_bits, (n + D - 1) / D);
-  const WindowPlan plan = make_plan(ci.fr_bits, c);
-  const size_t xb = 16u * ci.coord_words;
-  std::vector<unsigned char> h_part(D * plan.nwin * xb);
-  std::vector<int> rcs(D, GMSM_OK);
-  std::vector<std::string> errs(D);
   std::vector<SessionLease> leases(D);
+  std::vector<Shard> shards;
   for (size_t d = 0; d < D; d++) {
     const size_t lo = n * d / D, hi = n * (d + 1) / D;
     leases[d].acquire(curve, devs[d]);
-    if (int rc = session_prepare(*leases[d].S, curve, devs[d], hi - lo)) return rc;
+    Session& S = *leases[d].S;
+    if (int rc = session_prepare(S, curve, devs[d], hi - lo)) return rc;
+    shards.push_back({&S.pipe, S.d_points, points + lo * (ab / 8), scalars + lo * (size_t)(ci.scalar_bytes / 8), hi - lo});
   }
-  {
-    std::vector<std::thread> th;
-    for (size_t d = 0; d < D; d++) {
-      th.emplace_back([&, d]() {
-        const size_t lo = n * d / D, hi = n * (d + 1) / D;
-        Session& S = *leases[d].S;
-        rcs[d] = pipeline_run(S.pipe, S.d_points, points + lo * (ab / 8), scalars + lo * (size_t)(ci.scalar_bytes / 8), hi - lo, nullptr, c,
-                              h_part.data() + d * plan.nwin * xb);
-        if (rcs[d]) errs[d] = g_err;   // thread-local error text of the worker
-      });
-    }
-    for (auto& t : th) t.join();
-  }
-  for (size_t d = 0; d < D; d++)
-    if (rcs[d]) return set_err(rcs[d], "device %d: %s", devs[d], errs[d].c_str());
-  // join on the first device: per-window sum over the D shards, Horner, normalisation
-  Session& S0 = *leases[0].S;
-  if (int rc = join_partials(curve, S0.pipe, &S0.d_gather, &S0.gather_cap, h_part.data(), h_part.size(), (int)D, out_jac)) return rc;
+  if (int rc = run_shards(shards, c, out_jac)) return rc;
   int launches = 1;
   for (size_t d = 0; d < D; d++) launches += leases[d].S->pipe.last_launches;
   g_last_oneshot_launches = launches;
@@ -1270,20 +1208,19 @@ extern "C" int gmsm_bw6633_g2_multiexp(const uint64_t* p, const uint64_t* s, siz
 // ------------------------------------------------------------------------------------------
 extern "C" int gmsm_generate_multiples_device(gmsm_curve_t curve, const uint64_t* base_affine_host, uint64_t start, size_t n,
                                               void* d_out_points, void* stream) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
   if (n == 0) return GMSM_OK;
   if (int rc = set_device_of(d_out_points)) return rc;
-  void* d_base = nullptr;
-  const size_t ab = 8u * ci.coord_words;
-  CK(cudaMalloc(&d_base, ab));
+  DevBuf base;
+  const size_t ab = 8u * vt->ci.coord_words;
+  CK(cudaMalloc(&base.p, ab));
   cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t e = cudaMemcpyAsync(d_base, base_affine_host, ab, cudaMemcpyHostToDevice, st);
-  if (e != cudaSuccess) { cudaFree(d_base); return set_err(GMSM_ECUDA, "H2D base: %s", cudaGetErrorString(e)); }
-  int rc = vtable(curve)->generate(d_base, start, n, d_out_points, st);
+  cudaError_t e = cudaMemcpyAsync(base.p, base_affine_host, ab, cudaMemcpyHostToDevice, st);
+  if (e != cudaSuccess) return set_err(GMSM_ECUDA, "H2D base: %s", cudaGetErrorString(e));
+  int rc = vt->generate(base.p, start, n, d_out_points, st);
   e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  cudaFree(d_base);
   if (e != cudaSuccess) return set_err(GMSM_ECUDA, "generate_multiples: %s", cudaGetErrorString(e));
   return rc;
 }
@@ -1293,73 +1230,51 @@ extern "C" int gmsm_generate_multiples_device(gmsm_curve_t curve, const uint64_t
 // ------------------------------------------------------------------------------------------
 extern "C" int gmsm_batch_scalar_mul(gmsm_curve_t curve, const uint64_t* base_affine, const uint64_t* scalars, size_t n,
                                      uint64_t* out_points) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) return set_err(GMSM_ENODEV, "no CUDA device (%s); this engine has no CPU fallback", cudaGetErrorString(e));
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  if (int rc = use_device(default_device())) return rc;
   if (n == 0) return GMSM_OK;
   if (n > 0xFFFFFFF0ull) return set_err(GMSM_EINVAL, "n too large");
-  int device = 0;
-  if (const char* ev = getenv("GMSM_DEVICE")) device = atoi(ev);
-  CK(cudaSetDevice(device));
   // window width: on the GPU the doublings (fr.Bits of them) dominate whatever c is; c = 8 keeps the table
   // (2^7 .. 2^8 points) cache resident.  The result does not depend on c.
   const int c = 8;
-  const WindowPlan p = make_plan(ci.fr_bits, c);
+  const WindowPlan p = make_plan(vt->ci.fr_bits, c);
   const int maxc = std::max(p.c, p.last_c);
   const size_t tbl = (size_t)1 << (maxc - 1);
-  const size_t ab = 8u * ci.coord_words;
-  void *d_table = nullptr, *d_scalars = nullptr, *d_out = nullptr;
+  const size_t ab = 8u * vt->ci.coord_words, sb = (size_t)vt->ci.scalar_bytes;
+  DevBuf table, dsc, dout;
   cudaStream_t st = nullptr;
-  int rc = GMSM_OK;
-  auto cleanup = [&]() { cudaFree(d_table); cudaFree(d_scalars); cudaFree(d_out); if (st) cudaStreamDestroy(st); };
-  if (cudaMalloc(&d_table, tbl * ab) != cudaSuccess || cudaMalloc(&d_scalars, n * (size_t)ci.scalar_bytes) != cudaSuccess ||
-      cudaMalloc(&d_out, n * ab) != cudaSuccess || cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) {
-    cleanup();
+  if (cudaMalloc(&table.p, tbl * ab) != cudaSuccess || cudaMalloc(&dsc.p, n * sb) != cudaSuccess || cudaMalloc(&dout.p, n * ab) != cudaSuccess ||
+      cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess)
     return set_err(GMSM_ENOMEM, "gmsm_batch_scalar_mul: device allocation failed");
-  }
-  rc = gmsm_generate_multiples_device(curve, base_affine, 1, tbl, d_table, st);
+  int rc = gmsm_generate_multiples_device(curve, base_affine, 1, tbl, table.p, st);
   if (rc == GMSM_OK) {
-    cudaError_t ce = cudaMemcpyAsync(d_scalars, scalars, n * (size_t)ci.scalar_bytes, cudaMemcpyHostToDevice, st);
-    if (ce == cudaSuccess) rc = vtable(curve)->batch_scalar_mul(d_table, d_scalars, n, p.c, p.nwin, d_out, st);
-    if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpyAsync(out_points, d_out, n * ab, cudaMemcpyDeviceToHost, st);
+    cudaError_t ce = cudaMemcpyAsync(dsc.p, scalars, n * sb, cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess) rc = vt->batch_scalar_mul(table.p, dsc.p, n, p.c, p.nwin, dout.p, st);
+    if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpyAsync(out_points, dout.p, n * ab, cudaMemcpyDeviceToHost, st);
     if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaStreamSynchronize(st);
     if (ce != cudaSuccess) rc = set_err(GMSM_ECUDA, "gmsm_batch_scalar_mul: %s", cudaGetErrorString(ce));
   }
-  cleanup();
+  cudaStreamDestroy(st);
   return rc;
 }
 
 // ------------------------------------------------------------------------------------------
 // kzg.ToLagrangeG1 (ecc/<curve>/kzg/utils.go:25-64): inverse FFT over G1 points (lagrange_kernels.cuh)
 // ------------------------------------------------------------------------------------------
-static int lagrange_fr_field(int curve) {   // the scalar field of a pairing curve's G1 group, -1 for the other groups
-  switch (curve) {
-    case GMSM_BN254_G1: return GMSM_FR_BN254;
-    case GMSM_BLS12381_G1: return GMSM_FR_BLS12381;
-    case GMSM_BLS12377_G1: return GMSM_FR_BLS12377;
-    case GMSM_BLS24315_G1: return GMSM_FR_BLS24315;
-    case GMSM_BLS24317_G1: return GMSM_FR_BLS24317;
-    case GMSM_BW6633_G1: return GMSM_FR_BW6633;
-    case GMSM_BW6761_G1: return GMSM_FR_BW6761;
-  }
-  return -1;
-}
-
 extern "C" size_t gmsm_g1_to_lagrange_workspace_bytes(gmsm_curve_t curve, size_t n) {
-  return lagrange_fr_field(curve) < 0 ? 0 : n * gmsm_xyzz_bytes(curve);
+  const Group* g = group(curve);
+  return g && g->fr_field >= 0 ? n * gmsm_xyzz_bytes(curve) : 0;
 }
 
 // the argument checks of both entry points, before any device work: curve, then the reference's order (power of two, root)
 static int to_lagrange_args(int curve, size_t n, uint64_t* w_inv, uint64_t* n_inv) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) return set_err(GMSM_EINVAL, "unknown curve id %d", curve);
-  const int field = lagrange_fr_field(curve);
-  if (field < 0 || !vtable(curve)->to_lagrange)
+  const Group* g = group(curve);
+  if (!g) return set_err(GMSM_EINVAL, "unknown curve id %d", curve);
+  if (g->fr_field < 0 || !g->vt->to_lagrange)
     return set_err(GMSM_EINVAL, "ToLagrangeG1 is provided for the G1 groups of the pairing curves only (curve id %d)", curve);
   if (n == 0 || (n & (n - 1)) != 0) return set_err(GMSM_EINVAL, "len(coeffs) must be a power of 2");   // utils.go:26-28
-  if (int rc = fr_domain_inverses(field, n, w_inv, n_inv)) return rc;                                  // utils.go:33-36
+  if (int rc = fr_domain_inverses(g->fr_field, n, w_inv, n_inv)) return rc;                            // utils.go:33-36
   if (n > ((size_t)1 << LAG_MAX_LOG)) return set_err(GMSM_EINVAL, "len(coeffs) = %zu exceeds 2^%d", n, LAG_MAX_LOG);
   return GMSM_OK;
 }
@@ -1382,37 +1297,26 @@ extern "C" int gmsm_g1_to_lagrange(gmsm_curve_t curve, const uint64_t* points, s
   uint64_t w_inv[6], n_inv[6];
   if (int rc = to_lagrange_args(curve, n, w_inv, n_inv)) return rc;
   if (!points || !out) return set_err(GMSM_EINVAL, "null point array");
-  if (int rc = check_device(device)) return rc;
-  CK(cudaSetDevice(device));
+  if (int rc = use_device(device)) return rc;
   const size_t bytes = n * gmsm_affine_bytes(curve);
-  void *d_pts = nullptr, *d_work = nullptr;
+  DevBuf pts, work;
   cudaStream_t st = nullptr;
-  auto cleanup = [&]() { cudaFree(d_pts); cudaFree(d_work); if (st) cudaStreamDestroy(st); };
-  if (cudaMalloc(&d_pts, bytes) != cudaSuccess || cudaMalloc(&d_work, std::max<size_t>(gmsm_g1_to_lagrange_workspace_bytes(curve, n), 16)) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) {
-    cleanup();
+  if (cudaMalloc(&pts.p, bytes) != cudaSuccess || cudaMalloc(&work.p, std::max<size_t>(gmsm_g1_to_lagrange_workspace_bytes(curve, n), 16)) != cudaSuccess ||
+      cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess)
     return set_err(GMSM_ENOMEM, "gmsm_g1_to_lagrange: device allocation failed (n = %zu)", n);
-  }
   int rc = GMSM_OK;
-  cudaError_t ce = cudaMemcpyAsync(d_pts, points, bytes, cudaMemcpyHostToDevice, st);
-  if (ce == cudaSuccess) rc = gmsm_g1_to_lagrange_device(curve, d_pts, n, d_pts, d_work, st);
-  if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpyAsync(out, d_pts, bytes, cudaMemcpyDeviceToHost, st);
+  cudaError_t ce = cudaMemcpyAsync(pts.p, points, bytes, cudaMemcpyHostToDevice, st);
+  if (ce == cudaSuccess) rc = gmsm_g1_to_lagrange_device(curve, pts.p, n, pts.p, work.p, st);
+  if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpyAsync(out, pts.p, bytes, cudaMemcpyDeviceToHost, st);
   if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaStreamSynchronize(st);
   if (ce != cudaSuccess) rc = set_err(GMSM_ECUDA, "gmsm_g1_to_lagrange: %s", cudaGetErrorString(ce));
-  cleanup();
+  cudaStreamDestroy(st);
   return rc;
 }
 
 // ------------------------------------------------------------------------------------------
 // test hooks
 // ------------------------------------------------------------------------------------------
-namespace {
-struct DevBuf {   // frees on every exit path (the CK macro returns early on errors)
-  void* p = nullptr;
-  ~DevBuf() { if (p) cudaFree(p); }
-  template <class T> T* as() { return reinterpret_cast<T*>(p); }
-};
-}  // namespace
 extern "C" int gmsm_test_op(gmsm_curve_t curve, int op, const uint32_t* a, const uint32_t* b, uint32_t* out, size_t n) {
   int wa = 0, wb = 0, wo = 0;
   const GroupVTable* vt = vtable(curve);
@@ -1434,18 +1338,18 @@ extern "C" int gmsm_test_op(gmsm_curve_t curve, int op, const uint32_t* a, const
 }
 
 extern "C" int gmsm_test_digits(gmsm_curve_t curve, int c, const uint64_t* scalars, size_t n, uint32_t* out) {
-  CurveInfo ci;
-  if (!curve_info(curve, &ci)) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
   if (c < 2 || c > 24) return set_err(GMSM_EINVAL, "c out of range");
   if (n == 0) return GMSM_OK;
-  WindowPlan p = make_plan(ci.fr_bits, c);
+  WindowPlan p = make_plan(vt->ci.fr_bits, c);
   DevBuf bs, bo;
-  CK(cudaMalloc(&bs.p, n * (size_t)ci.scalar_bytes));
+  CK(cudaMalloc(&bs.p, n * (size_t)vt->ci.scalar_bytes));
   CK(cudaMalloc(&bo.p, n * (size_t)p.nwin * 4));
   void* ds = bs.p;
   uint32_t* dout = bo.as<uint32_t>();
-  CK(cudaMemcpy(ds, scalars, n * (size_t)ci.scalar_bytes, cudaMemcpyHostToDevice));
-  if (int rc = vtable(curve)->digits_dump(ds, n, p.c, p.nwin, dout)) return rc;
+  CK(cudaMemcpy(ds, scalars, n * (size_t)vt->ci.scalar_bytes, cudaMemcpyHostToDevice));
+  if (int rc = vt->digits_dump(ds, n, p.c, p.nwin, dout)) return rc;
   CK(cudaDeviceSynchronize());
   CK(cudaMemcpy(out, dout, n * (size_t)p.nwin * 4, cudaMemcpyDeviceToHost));
   return GMSM_OK;
