@@ -27,6 +27,8 @@ SYMBOLS = [
     "gmsm_ctx_set_profiling", "gmsm_ctx_last_stage_ms", "gmsm_generate_multiples_device", "gmsm_batch_scalar_mul", "gmsm_g1_decode", "gmsm_g1_decode_device", "gmsm_fft_fr_bytes", "gmsm_fft_domain_create", "gmsm_fft_domain_free", "gmsm_fft_domain_cardinality",
     "gmsm_fft_domain_constants", "gmsm_fft", "gmsm_fft_inverse", "gmsm_fft_device", "gmsm_fft_bit_reverse_device",
     "gmsm_fr_poly_workspace_bytes", "gmsm_fr_poly_div_x_minus_a_device", "gmsm_fr_poly_fold_device", "gmsm_fr_poly_lincomb_device",
+    "gmsm_fr_batch_invert_device", "gmsm_fr_permutation_workspace_bytes", "gmsm_fr_permutation_accumulate_device",
+    "gmsm_fft_permutation_numerator_device",
     "gmsm_g1_to_lagrange_workspace_bytes", "gmsm_g1_to_lagrange", "gmsm_g1_to_lagrange_device", "gmsm_test_op", "gmsm_test_digits",
 ]
 
@@ -109,6 +111,11 @@ def lib() -> ctypes.CDLL:
     L.gmsm_fr_poly_div_x_minus_a_device.argtypes = [i32, vp, sz, vp, vp, vp, vp, vp]
     L.gmsm_fr_poly_fold_device.argtypes = [i32, vp, vp, sz, vp, vp, sz, vp]
     L.gmsm_fr_poly_lincomb_device.argtypes = [i32, vp, vp, vp, vp, vp, sz, vp, sz, i32, vp]
+    L.gmsm_fr_batch_invert_device.argtypes = [i32, vp, sz, vp, vp]
+    L.gmsm_fr_permutation_workspace_bytes.restype = sz
+    L.gmsm_fr_permutation_workspace_bytes.argtypes = [i32, sz]
+    L.gmsm_fr_permutation_accumulate_device.argtypes = [i32, vp, vp, sz, vp, vp, vp, vp]
+    L.gmsm_fft_permutation_numerator_device.argtypes = [vp, vp, vp, vp, sz, vp, vp, vp, vp]
     L.gmsm_g1_to_lagrange_workspace_bytes.restype = sz
     L.gmsm_g1_to_lagrange_workspace_bytes.argtypes = [i32, sz]
     L.gmsm_g1_to_lagrange.argtypes = [i32, vp, sz, i32, vp]

@@ -19,6 +19,10 @@
 //   dividePolyByXminusA           ecc/bn254/kzg/kzg.go:567-582
 //   the gamma-fold of BatchOpenSinglePoint   ecc/bn254/kzg/kzg.go:302-319
 //   the strided linear combinations of shplonk.BatchOpen / fflonk.Fold (gmsm_fr_poly_lincomb_device)
+// and the Fr steps of permutation.Prove (kernels and schedule in perm_kernels.cuh):
+//   fr.BatchInvert                                ecc/bn254/fr/element.go:658-687
+//   evaluateAccumulationPolynomialBitReversed     ecc/bn254/fr/permutation/permutation.go:52-75
+//   the quotient numerator and its omega-fold     ecc/bn254/fr/permutation/permutation.go:78-121, 206-214
 #include <cuda_runtime.h>
 
 #include <cstdio>
@@ -33,6 +37,7 @@ using namespace gmsm;
 
 #include "fft_kernels.cuh"
 #include "poly_kernels.cuh"
+#include "perm_kernels.cuh"
 
 namespace {
 
@@ -404,6 +409,111 @@ extern "C" int gmsm_fr_poly_lincomb_device(int fr_field, const void* const* d_po
     std::vector<uint64_t> len(lens, lens + k), str(strides, strides + k), off(offsets, offsets + k);
     poly_lincomb_schedule<P>(reinterpret_cast<const F* const*>(d_polys), len.data(), s.data(), str.data(), off.data(), k,
                              accumulate ? 1 : 0, poly_fold_launcher<P>(d_out, out_len, stream));
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+// ---- fr.BatchInvert and the Fr steps of permutation.Prove (permutation.go:52-121) on device vectors ----
+
+namespace {
+
+bool overlaps(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
+  const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
+  return a0 < b0 + b_bytes && b0 < a0 + a_bytes;
+}
+
+// blocks of the tile inversion kernels (k_fr_batch_invert, k_perm_ratio, k_perm_numerator) over n elements
+unsigned perm_inv_tiles(uint64_t n) { return (unsigned)(((n - 1) >> PERM_INV_LOG_T) + 1); }
+
+template <class P>
+bool read_reduced(const uint64_t* limbs, Fp<P>* out) {
+  memcpy(out->l, limbs, sizeof(Fp<P>));
+  return host_is_reduced(*out);
+}
+
+}  // namespace
+
+extern "C" int gmsm_fr_batch_invert_device(int fr_field, const void* d_a, size_t n, void* d_out, void* stream) {
+  const size_t fb = gmsm_fft_fr_bytes(fr_field);
+  if (!fb) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0) return set_err(GMSM_EINVAL, "empty vector (n = 0)");
+  if (!d_a || !d_out) return set_err(GMSM_EINVAL, "null vector");
+  if (d_out != d_a && overlaps(d_a, n * fb, d_out, n * fb)) return set_err(GMSM_EINVAL, "the output must equal the input or not overlap it");
+  if (((n - 1) >> PERM_INV_LOG_T) >= 0x7fffffffull) return set_err(GMSM_EINVAL, "vector too large (n = %zu)", n);
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    k_fr_batch_invert<P><<<perm_inv_tiles(n), PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), (cudaStream_t)stream>>>(
+        reinterpret_cast<const F*>(d_a), n, PERM_INV_LOG_T, reinterpret_cast<F*>(d_out));
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" size_t gmsm_fr_permutation_workspace_bytes(int fr_field, size_t n) {
+  return gmsm_fr_poly_workspace_bytes(fr_field, n);   // the carry levels of the prefix product: the tile shape of the opening scan
+}
+
+extern "C" int gmsm_fr_permutation_accumulate_device(int fr_field, const void* d_t1, const void* d_t2, size_t n, const uint64_t* epsilon,
+                                                     void* d_z, void* d_work, void* stream) {
+  const size_t fb = gmsm_fft_fr_bytes(fr_field);
+  if (!fb) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0 || (n & (n - 1))) return set_err(GMSM_EINVAL, "n (%zu) must be a power of 2", n);
+  if (!d_t1 || !d_t2 || !d_z || !epsilon) return set_err(GMSM_EINVAL, "null vector or epsilon");
+  if (overlaps(d_z, n * fb, d_t1, n * fb) || overlaps(d_z, n * fb, d_t2, n * fb)) return set_err(GMSM_EINVAL, "z must not overlap t1 or t2");
+  if (!d_work && gmsm_fr_permutation_workspace_bytes(fr_field, n))
+    return set_err(GMSM_EINVAL, "null workspace (gmsm_fr_permutation_workspace_bytes)");
+  if (((n - 1) >> PERM_INV_LOG_T) >= 0x7fffffffull) return set_err(GMSM_EINVAL, "vector too large (n = %zu)", n);
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    F eps;
+    if (!read_reduced(epsilon, &eps)) return set_err(GMSM_EINVAL, "epsilon is not a reduced fr.Element");
+    cudaStream_t st = (cudaStream_t)stream;
+    F* z = reinterpret_cast<F*>(d_z);
+    k_perm_ratio<P><<<perm_inv_tiles(n), PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), st>>>(
+        reinterpret_cast<const F*>(d_t1), reinterpret_cast<const F*>(d_t2), n, eps, PERM_INV_LOG_T, z);
+    constexpr int log_l = poly_log_l<P>(), log_b = poly_log_b<P>();
+    const size_t smem = poly_smem_bytes<P>(log_l, log_b);
+    perm_prefix_schedule<P>(
+        z, n, reinterpret_cast<F*>(d_work), log_l, log_b,
+        [&](const F* x, uint64_t m, F* heads, uint64_t tiles) {
+          k_perm_prod_heads<P><<<(unsigned)tiles, 1u << log_b, smem, st>>>(x, m, log_l, heads);
+        },
+        [&](F* x, uint64_t m, const F* carry, uint64_t tiles) {
+          k_perm_prod_write<P><<<(unsigned)tiles, 1u << log_b, smem, st>>>(x, m, log_l, carry);
+        });
+    // natural order -> the bit-reversed layout of the reference
+    int logn = 0;
+    while (((uint64_t)1 << logn) < n) logn++;
+    k_fft_bit_reverse<P><<<(unsigned)std::min<uint64_t>((n + 255) / 256, GMSM_NUM_SMS * 32u), 256, 0, st>>>(z, n, logn);
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fft_permutation_numerator_device(gmsm_fft_domain_t* d, const void* d_lt1, const void* d_lt2, const void* d_lz, size_t n,
+                                                     const uint64_t* epsilon, const uint64_t* omega, void* d_out, void* stream) {
+  if (!d) return set_err(GMSM_EINVAL, "null domain");
+  if (n != d->n) return set_err(GMSM_EINVAL, "len(a) = %zu must equal the domain cardinality %llu", n, (unsigned long long)d->n);
+  if (!d_lt1 || !d_lt2 || !d_lz || !d_out || !epsilon || !omega) return set_err(GMSM_EINVAL, "null vector or challenge");
+  const size_t bytes = n * 8 * (size_t)d->words;
+  if (overlaps(d_out, bytes, d_lt1, bytes) || overlaps(d_out, bytes, d_lt2, bytes) || overlaps(d_out, bytes, d_lz, bytes))
+    return set_err(GMSM_EINVAL, "the output must not overlap lt1, lt2 or lz");
+  std::lock_guard<std::mutex> lk(d->mu);
+  CK(cudaSetDevice(d->device));
+  return with_fr(d->field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    PermNumConsts<P> k;
+    if (!read_reduced(epsilon, &k.eps)) return set_err(GMSM_EINVAL, "epsilon is not a reduced fr.Element");
+    if (!read_reduced(omega, &k.omega)) return set_err(GMSM_EINVAL, "omega is not a reduced fr.Element");
+    memcpy(k.g.l, d->consts[3], sizeof(F));
+    k.tn_inv = fp_inv(fp_sub(host_pow2k(k.g, d->logn), F::one()));   // (g^n - 1)^-1, permutation.go:208
+    k_perm_numerator<P><<<perm_inv_tiles(n), PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), (cudaStream_t)stream>>>(
+        reinterpret_cast<const F*>(d_lt1), reinterpret_cast<const F*>(d_lt2), reinterpret_cast<const F*>(d_lz), n, d->logn, k,
+        reinterpret_cast<const F*>(d->d_tw), PERM_INV_LOG_T, reinterpret_cast<F*>(d_out));
     CK(cudaGetLastError());
     return GMSM_OK;
   });

@@ -251,6 +251,28 @@ int gmsm_fr_poly_lincomb_device(int fr_field, const void* const* d_polys, const 
                                 const size_t* strides, const size_t* offsets, size_t k, void* d_out, size_t out_len, int accumulate,
                                 void* stream);
 
+/* ---- the Fr steps of permutation.Prove (ecc/bn254/fr/permutation/permutation.go; the same for the other six scalar fields)
+ * and fr.BatchInvert on device vectors, with the conventions of the gmsm_fr_poly_* block above (vectors on the current device,
+ * ordered on `stream`, nothing allocated inside a call, reduced Montgomery host scalars).  GMSM_EINVAL: unknown field, n = 0, an
+ * unreduced scalar, a null vector, buffers that overlap where this is not allowed. ---- */
+/* d_out[i] = d_a[i]^-1 for i < n, zero -> zero (fr.BatchInvert, fr/element.go:658-687); d_out may equal d_a (in place) but
+ * must not overlap it otherwise */
+int gmsm_fr_batch_invert_device(int fr_field, const void* d_a, size_t n, void* d_out, void* stream);
+/* bytes of device workspace gmsm_fr_permutation_accumulate_device needs for n elements (0: none; 0 for an unknown field) */
+size_t gmsm_fr_permutation_workspace_bytes(int fr_field, size_t n);
+/* evaluateAccumulationPolynomialBitReversed (permutation.go:52-75): d_z[rev(k)] = prod_{j<k} (eps - t1[j]) (eps - t2[j])^-1
+ * with zero -> zero inversion (the reference's entries past the first eps = t2[k-1] are zero), d_z[0] = 1; n a power of two.
+ * d_z must not overlap d_t1 or d_t2, which are left unchanged. */
+int gmsm_fr_permutation_accumulate_device(int fr_field, const void* d_t1, const void* d_t2, size_t n, const uint64_t* epsilon,
+                                          void* d_z, void* d_work, void* stream);
+/* the quotient numerator of permutation.Prove (evaluateFirstPartNumReverse, evaluateSecondPartNumReverse and the omega-fold,
+ * permutation.go:78-121, 206-214) from the bit-reversed coset DIF outputs lt1, lt2, lz: with i = rev(p), w the domain's generator
+ * and g its FrMultiplicativeGen, d_out[p] = (omega (lz[p] - 1) (g^n - 1) / (g w^i - 1) + (eps - lt2[p]) lz[rev(i + 1 mod n)] -
+ * (eps - lt1[p]) lz[p]) / (g^n - 1).  n must equal the domain cardinality; d_out must not overlap the inputs, which are left
+ * unchanged. */
+int gmsm_fft_permutation_numerator_device(gmsm_fft_domain_t* domain, const void* d_lt1, const void* d_lt2, const void* d_lz, size_t n,
+                                          const uint64_t* epsilon, const uint64_t* omega, void* d_out, void* stream);
+
 /* ---- kzg.ToLagrangeG1 (ecc/bn254/kzg/utils.go:25-64; the same for the other pairing curves): the canonical SRS [tau^i]G in,
  * its Lagrange form [L_i(tau)]G out, by an inverse FFT over G1 points on the device.  Curves: the G1 groups of bn254, bls12-381,
  * bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761 (others: GMSM_EINVAL).  Points are the reference's in-memory G1Affine
