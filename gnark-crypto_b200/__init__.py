@@ -3,10 +3,13 @@
 Layout:
   csrc/        sm_90a CUDA kernels + the C ABI (include/gmsm.h) -> libgmsm.so (built in-tree)
   _native.py   ctypes loader of libgmsm.so (fails loudly when the library or a GPU is missing)
+  curves.py    the one curve table: the thirteen MultiExp groups, the seven pairing curves of the prover, the fr.Element codec
   multiexp.py  host-side mirror of the reference interface for this path:
                G1Affine/G1Jac/G2Affine/G2Jac .MultiExp(points, scalars, MultiExpConfig)
                (ecc/bn254/multiexp.go:20,32,345,357; ecc/ecc.go:107-110) + the device-level Engine
   dist.py      multi-GPU: one process per GPU, shard points/scalars, all-gather the per-window partials
+  fft.py, kzg.py, shplonk.py, fflonk.py, permutation.py, transcript.py: the Fr FFT and the KZG provers; kzg._DevicePoly is
+               the one caller of the library's device Fr polynomial entry points
 """
 from . import _native  # noqa: F401
 from .multiexp import (  # noqa: F401

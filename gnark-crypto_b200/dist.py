@@ -99,16 +99,14 @@ class ShardedMultiExp:
         import numpy as np
 
         from . import _native
-        from .multiexp import MultiExpError
+        from .multiexp import _check
 
         torch = self.engine.torch
         eng = self.engine
         n_local = h_scalars_np.size // eng.sw
         part = np.empty(eng.partials_bytes // 8, dtype=np.uint64)
-        rc = _native.lib().gmsm_multiexp_window_sums(eng.cid, h_points_np.ctypes.data, h_scalars_np.ctypes.data, n_local, eng.c,
-                                                     eng.device, part.ctypes.data)
-        if rc != 0:
-            raise MultiExpError(_native.last_error())
+        _check(_native.lib().gmsm_multiexp_window_sums(eng.cid, h_points_np.ctypes.data, h_scalars_np.ctypes.data, n_local, eng.c,
+                                                       eng.device, part.ctypes.data))
         local = torch.from_numpy(part.view(np.int64)).to(torch.device("cuda", eng.device))
         allp = gather_partials(local, self.world, self.group)
         return eng.finalize(allp, self.world)

@@ -9,11 +9,8 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import kzg, shplonk
-from .kzg import ErrInvalidPolynomialSize, _fr_decode, _fr_encode
+from .curves import _fr_decode, _fr_encode, _params
 from .multiexp import MultiExpError
-
-# fft.GeneratorFullMultiplicativeGroup (fr/fft/domain.go:56-60 of each curve)
-_MULT_GEN = {"bn254": 5, "bls12381": 7, "bls12377": 22, "bls24315": 7, "bls24317": 7, "bw6633": 13, "bw6761": 15}
 
 
 class ErrRootsOne(MultiExpError):
@@ -48,16 +45,16 @@ def _next_divisor_r_minus_one(i: int, r: int) -> int:
 
 def _ith_root_one(i: int, curve: str) -> int:
     """getIthRootOne (fflonk.go:213-230): GeneratorFullMultiplicativeGroup^((r - 1) / i)"""
-    c = curve.split("_")[0]
-    r = kzg._params(c).r
+    cp = _params(curve)
+    r = cp.r
     if (r - 1) % i != 0:
         raise ErrRootsOne("fr does not contain all the t-th roots of 1")
-    return pow(_MULT_GEN[c], (r - 1) // i, r)
+    return pow(cp.mult_gen, (r - 1) // i, r)
 
 
 def _extend_set(points: list, t: int, curve: str) -> list:
     """extendSet (fflonk.go:255-271): [p0, omega p0, .., omega^(t-1) p0, p1, ...]"""
-    r = kzg._params(curve).r
+    r = _params(curve).r
     omega = _ith_root_one(t, curve)
     out = []
     for p in points:
@@ -71,7 +68,7 @@ def _extend_set(points: list, t: int, curve: str) -> list:
 def Fold(p, curve: str) -> np.ndarray:
     """Fold (fflonk.go:52-71) on the host: F[j t + i] = p[i][j], t = getNextDivisorRMinusOne(len(p)), t * max len(p[i])
     coefficients as a (n, fr.Limbs) uint64 array"""
-    cp = kzg._params(curve)
+    cp = _params(curve)
     w = cp.fr_words
     t = _next_divisor_r_minus_one(len(p), cp.r)
     hp = [kzg._host_poly(x, w) for x in p]
@@ -84,7 +81,7 @@ def Fold(p, curve: str) -> np.ndarray:
 def FoldAndCommit(p, pk: kzg.ProvingKey, *nbTasks: int) -> np.ndarray:
     """FoldAndCommit (fflonk.go:43-47): kzg.Commit(Fold(p), pk).  On a single-device key the interleave is one
     gmsm_fr_poly_lincomb_device (stride t) into device memory that feeds the MultiExp."""
-    cp = kzg._params(pk.curve)
+    cp = _params(pk.curve)
     w = cp.fr_words
     if pk.device < 0:
         return kzg.Commit(Fold(p, pk.curve), pk, *nbTasks)
@@ -93,10 +90,9 @@ def FoldAndCommit(p, pk: kzg.ProvingKey, *nbTasks: int) -> np.ndarray:
     t = _next_divisor_r_minus_one(len(p), cp.r)
     lens = [kzg._poly_len(x, w) for x in p]
     size = t * max(lens)
-    if size == 0 or size > pk.G1.shape[0]:
-        raise ErrInvalidPolynomialSize(shplonk._SIZE_ERR)
+    kzg._check_size(size, 1, pk.G1.shape[0])
     with torch.cuda.device(pk.device):
-        dp = kzg._DevicePoly(pk, 0)
+        dp = kzg._DevicePoly(pk.curve, pk.device, 0)
         ins = [(kzg._device_poly(x, w, pk.device), n, i) for i, (x, n) in enumerate(zip(p, lens)) if n]
         d_F = dp.empty(size)
         dp.lincomb([d for d, _, _ in ins], [n for _, n, _ in ins], _fr_encode([1] * len(ins), cp.r), [t] * len(ins),
@@ -109,7 +105,7 @@ def BatchOpen(p, digests, points, hf, pk: kzg.ProvingKey, *dataTranscript: bytes
     left unmodified) is opened on the powers s^t of points[j]; digests[j] = FoldAndCommit(p[j])."""
     if len(p) != len(points):
         raise ErrNbPolynomialsNbPoints("the number of packs of polynomials should be the same as the number of pack of points")
-    cp = kzg._params(pk.curve)
+    cp = _params(pk.curve)
     r, w = cp.r, cp.fr_words
     ts = [_next_divisor_r_minus_one(len(pack), r) for pack in p]
     base = [shplonk._decode_points(S, r) for S in points]

@@ -9,10 +9,10 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native
-from .multiexp import MultiExpError
+from .curves import CURVE_PARAMS
+from .multiexp import MultiExpError, _check, _handle
 
 DIT, DIF = 0, 1  # fft.Decimation
-_FIELDS = {"bn254": 0, "bls12381": 1, "bls12377": 2, "bls24315": 3, "bls24317": 4, "bw6633": 5, "bw6761": 6}
 
 
 class Domain:
@@ -20,16 +20,15 @@ class Domain:
 
     def __init__(self, curve: str, m: int, shift: np.ndarray = None, device: int = 0):
         L = _native.lib()
-        if curve not in _FIELDS:
-            raise MultiExpError("unknown curve %r (FFT over Fr: %s)" % (curve, ", ".join(_FIELDS)))
-        self.words = int(L.gmsm_fft_fr_bytes(_FIELDS[curve])) // 8
+        if curve not in CURVE_PARAMS:
+            raise MultiExpError("unknown curve %r (FFT over Fr: %s)" % (curve, ", ".join(CURVE_PARAMS)))
+        fr_id = CURVE_PARAMS[curve].fr_id
+        self.words = int(L.gmsm_fft_fr_bytes(fr_id)) // 8
         sp = None
         if shift is not None:
             shift = np.ascontiguousarray(shift, dtype=np.uint64).reshape(self.words)
             sp = shift.ctypes.data
-        self._h = L.gmsm_fft_domain_create(_FIELDS[curve], int(m), sp, device)
-        if not self._h:
-            raise MultiExpError(_native.last_error())
+        self._h = _handle(L.gmsm_fft_domain_create(fr_id, int(m), sp, device))
         self.device = device
         self.Cardinality = int(L.gmsm_fft_domain_cardinality(self._h))
         c = np.zeros(5 * self.words, dtype=np.uint64)
@@ -47,30 +46,22 @@ class Domain:
 
     def FFT(self, a: np.ndarray, decimation: int, OnCoset: bool = False):
         a = self._vec(a)
-        rc = _native.lib().gmsm_fft(self._h, a.ctypes.data, self.Cardinality, int(decimation), 1 if OnCoset else 0)
-        if rc:
-            raise MultiExpError(_native.last_error())
+        _check(_native.lib().gmsm_fft(self._h, a.ctypes.data, self.Cardinality, int(decimation), 1 if OnCoset else 0))
         return a
 
     def FFTInverse(self, a: np.ndarray, decimation: int, OnCoset: bool = False):
         a = self._vec(a)
-        rc = _native.lib().gmsm_fft_inverse(self._h, a.ctypes.data, self.Cardinality, int(decimation), 1 if OnCoset else 0)
-        if rc:
-            raise MultiExpError(_native.last_error())
+        _check(_native.lib().gmsm_fft_inverse(self._h, a.ctypes.data, self.Cardinality, int(decimation), 1 if OnCoset else 0))
         return a
 
     # device tensors (torch int64 views of the same layout)
     def fft_device(self, d_a, inverse: bool, decimation: int, coset: bool = False, stream=None):
-        rc = _native.lib().gmsm_fft_device(self._h, d_a.data_ptr(), self.Cardinality, 1 if inverse else 0, int(decimation),
-                                           1 if coset else 0, stream)
-        if rc:
-            raise MultiExpError(_native.last_error())
+        _check(_native.lib().gmsm_fft_device(self._h, d_a.data_ptr(), self.Cardinality, 1 if inverse else 0, int(decimation),
+                                             1 if coset else 0, stream))
         return d_a
 
     def bit_reverse_device(self, d_a, stream=None):
-        rc = _native.lib().gmsm_fft_bit_reverse_device(self._h, d_a.data_ptr(), self.Cardinality, stream)
-        if rc:
-            raise MultiExpError(_native.last_error())
+        _check(_native.lib().gmsm_fft_bit_reverse_device(self._h, d_a.data_ptr(), self.Cardinality, stream))
         return d_a
 
     def close(self):

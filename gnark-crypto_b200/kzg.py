@@ -24,8 +24,9 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _native
-from .fft import _FIELDS
-from .multiexp import CURVES, BatchScalarMultiplication, MultiExpConfig, MultiExpError, ResidentBases, _check, _words
+from .curves import CURVE_PARAMS, CurveParams  # noqa: F401  (kzg's names for the curve table)
+from .curves import CURVES, GROUPS, _challenge, _curve, _fr_decode, _fr_encode, _fr_marshal, _g1_name, _params, _reduced
+from .multiexp import BatchScalarMultiplication, MultiExpConfig, MultiExpError, ResidentBases, _check
 from .transcript import Transcript
 
 MARKER = 0xDEADBEEF  # utils/unsafe/dump_slice.go:78
@@ -33,6 +34,12 @@ MARKER = 0xDEADBEEF  # utils/unsafe/dump_slice.go:78
 
 class ErrInvalidPolynomialSize(MultiExpError):
     """kzg.ErrInvalidPolynomialSize (kzg.go:24)"""
+
+
+def _check_size(n: int, n_min: int, n_max: int) -> None:
+    """the refusal of kzg.Commit (kzg.go:160-162) of a polynomial that is empty or larger than the SRS, with the caller's bounds"""
+    if not n_min <= n <= n_max:
+        raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
 
 
 def write_slice(w, points: np.ndarray) -> None:
@@ -75,8 +82,8 @@ class ProvingKey:
     """kzg.ProvingKey{G1 []G1Affine} (kzg.go:38-41) with the bases resident in HBM"""
 
     def __init__(self, curve: str, g1_points: np.ndarray, device: int = 0, window_tables: bool = False):
-        self.curve = curve + "_g1" if not curve.endswith("_g1") else curve
-        self.words = 2 * _words(CURVES[self.curve])
+        self.curve = _g1_name(curve)
+        self.words = 2 * GROUPS[self.curve].words
         self.G1 = np.ascontiguousarray(g1_points, dtype=np.uint64).reshape(-1, self.words)
         self.device = device       # -1: sharded over GMSM_DEVICES (host scalars only)
         self._bases = ResidentBases(self.curve, self.G1, device)
@@ -87,8 +94,7 @@ class ProvingKey:
     def from_dump(cls, curve: str, r, max_pk_points: int = 0, device: int = 0):
         """the marker + slice tail of SRS.ReadDump (marshal.go:98-115); `r` positioned at the marker"""
         read_marker(r)
-        cname = curve + "_g1" if not curve.endswith("_g1") else curve
-        pts = read_slice(r, 2 * _words(CURVES[cname]), max_pk_points)
+        pts = read_slice(r, 2 * GROUPS[_g1_name(curve)].words, max_pk_points)
         return cls(curve, pts, device)
 
     @classmethod
@@ -108,87 +114,7 @@ def new_srs_g1(curve: str, size: int, alpha: int, generator: np.ndarray, r_modul
     for _ in range(size):
         alphas.append(a)
         a = a * alpha % r_modulus
-    cname = curve + "_g1" if not curve.endswith("_g1") else curve
-    return BatchScalarMultiplication(cname, generator, encode_scalars(alphas))
-
-
-_TWO_BIT = dict(mask=0b11 << 6, unc=0b00 << 6, unc_inf=None, small=0b10 << 6, large=0b11 << 6, inf=0b01 << 6)
-_THREE_BIT = dict(mask=0b111 << 5, unc=0b000 << 5, unc_inf=0b010 << 5, small=0b100 << 5, large=0b101 << 5, inf=0b110 << 5)
-
-
-@dataclass(frozen=True)
-class CurveParams:
-    """What the prover and the point codec need of one pairing curve.  fr.Element / fp.Element hold v * 2^(64 * words) mod
-    the modulus (Montgomery form, little-endian u64 limbs); fr.Bytes / fp.Bytes = 8 * words (fr|fp/element.go:36-49)."""
-
-    fr_words: int           # fr.Limbs
-    fp_words: int           # fp.Limbs
-    r: int                  # scalar-field modulus
-    q: int                  # base-field modulus
-    b: int                  # y^2 = x^3 + b, as an integer mod q
-    flags: dict             # flag bits of the most significant byte of a serialised point (marshal.go:25-34)
-
-    @property
-    def fr_bytes(self) -> int:
-        return 8 * self.fr_words
-
-    @property
-    def fp_bytes(self) -> int:
-        return 8 * self.fp_words
-
-
-_Q_BW6761 = int("122E824FB83CE0AD187C94004FAFF3EB926186A81D14688528275EF8087BE41707BA638E584E91903CEBAFF25B423048689C8ED12F9FD9071DCD3DC73EBF"
-                "F2E98A116C25667A8F8160CF8AEEAF0A437E6913E6870000082F49D00000000008B", 16)
-# one entry per curve: fr/element.go and fp/element.go (q, Limbs), the curve's .go file (b), marshal.go (flags)
-CURVE_PARAMS = {
-    "bn254": CurveParams(4, 4, 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001,
-                         0x30644E72E131A029B85045B68181585D97816A916871CA8D3C208C16D87CFD47, 3, _TWO_BIT),
-    "bls12381": CurveParams(4, 6, 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001,
-                            0x1A0111EA397FE69A4B1BA7B6434BACD764774B84F38512BF6730D2A0F6B0F6241EABFFFEB153FFFFB9FEFFFFFFFFAAAB, 4, _THREE_BIT),
-    "bls12377": CurveParams(4, 6, 0x12AB655E9A2CA55660B44D1E5C37B00159AA76FED00000010A11800000000001,
-                            0x01AE3A4617C510EAC63B05C06CA1493B1A22D9F300F5138F1EF3622FBA094800170B5D44300000008508C00000000001, 1, _THREE_BIT),
-    "bls24315": CurveParams(4, 5, 0x196DEAC24A9DA12B25FC7EC9CF927A98C8C480ECE644E36419D0C5FD00C00001,
-                            0x4C23A02B586D650D3F7498BE97C5EAFDEC1D01AA27A1AE0421EE5DA52BDE5026FE802FF40300001, 1, _THREE_BIT),
-    "bls24317": CurveParams(4, 5, 0x443F917EA68DAFC2D0B097F28D83CD491CD1E79196BF0E7AF000000000000001,
-                            0x1058CA226F60892CF28FC5A0B7F9D039169A61E684C73446D6F339E43424BF7E8D512E565DAB2AAB, 4, _THREE_BIT),
-    "bw6633": CurveParams(5, 10, 0x4C23A02B586D650D3F7498BE97C5EAFDEC1D01AA27A1AE0421EE5DA52BDE5026FE802FF40300001,
-                          int("126633CC0F35F63FC1A174F01D72AB5A8FCD8C75D79D2C74E59769AD9BBDA2F8152A6C0FADEA490B8DA9F5E83F57C497E0E8850EDBDA40"
-                              "7D7B5CE7AB839C2253D369BD31147F73CD74916EA4570000D", 16), 4, _THREE_BIT),
-    "bw6761": CurveParams(6, 12, 0x01AE3A4617C510EAC63B05C06CA1493B1A22D9F300F5138F1EF3622FBA094800170B5D44300000008508C00000000001,
-                          _Q_BW6761, _Q_BW6761 - 1, _THREE_BIT),            # b = -1 (bw6-761.go)
-}
-# views of the table by field, kept for callers of the earlier per-constant dictionaries
-FR_MODULUS = {c: p.r for c, p in CURVE_PARAMS.items()}
-FP_MODULUS = {c: p.q for c, p in CURVE_PARAMS.items()}
-CURVE_B = {c: p.b for c, p in CURVE_PARAMS.items()}
-_FLAGS = {c: p.flags for c, p in CURVE_PARAMS.items()}
-
-
-def _params(curve: str) -> CurveParams:
-    return CURVE_PARAMS[curve.split("_")[0]]
-
-
-def _limbs(modulus: int) -> int:
-    """u64 limbs of an element mod `modulus` (fr.Limbs / fp.Limbs: the modulus' bit length rounded up to 64)"""
-    return (modulus.bit_length() + 63) // 64
-
-
-def _fr_decode(limbs: np.ndarray, r: int) -> list:
-    """Montgomery limbs -> regular integers"""
-    L = _limbs(r)
-    rinv = pow(1 << (64 * L), -1, r)
-    a = np.ascontiguousarray(limbs, dtype=np.uint64).reshape(-1, L)
-    return [sum(int(x[i]) << (64 * i) for i in range(L)) * rinv % r for x in a]
-
-
-def _fr_encode(vals, r: int) -> np.ndarray:
-    L = _limbs(r)
-    out = np.empty((len(vals), L), dtype=np.uint64)
-    m64 = (1 << 64) - 1
-    for i, v in enumerate(vals):
-        m = (v << (64 * L)) % r
-        out[i] = [(m >> (64 * k)) & m64 for k in range(L)]
-    return out
+    return BatchScalarMultiplication(_g1_name(curve), generator, encode_scalars(alphas))
 
 
 def _eval(p: list, point: int, r: int) -> int:
@@ -241,9 +167,11 @@ def _device_poly(p, words: int, device: int):
     return torch.from_numpy(h).to(torch.device("cuda", device))
 
 
-def _reduced(limbs, r: int) -> np.ndarray:
-    """Montgomery limbs of an fr.Element, reduced mod r (the device takes reduced elements only)"""
-    return _fr_encode([_fr_decode(limbs, r)[0]], r)[0]
+def _stream(device):
+    """the current torch stream of `device`, which orders the work of a call"""
+    import torch
+
+    return torch.cuda.current_stream(device).cuda_stream
 
 
 def _digest(jac: np.ndarray, w: int) -> np.ndarray:
@@ -251,16 +179,17 @@ def _digest(jac: np.ndarray, w: int) -> np.ndarray:
 
 
 class _DevicePoly:
-    """gmsm_fr_poly_* of one proving key's curve on its device, ordered on the device's current torch stream"""
+    """the gmsm_fr_* entry points of one curve's scalar field on one device, ordered on the device's current torch stream, with a
+    workspace for polynomials of up to max_len coefficients"""
 
-    def __init__(self, pk: ProvingKey, max_len: int):
+    def __init__(self, curve: str, device: int, max_len: int):
         import torch
 
         self.torch = torch
-        self.field = _FIELDS[pk.curve.split("_")[0]]
-        self.words = _params(pk.curve).fr_words
-        self.dev = torch.device("cuda", pk.device)
-        self.stream = torch.cuda.current_stream(self.dev).cuda_stream
+        self.field = _params(curve).fr_id
+        self.words = _params(curve).fr_words
+        self.dev = torch.device("cuda", device)
+        self.stream = _stream(self.dev)
         ws = int(_native.lib().gmsm_fr_poly_workspace_bytes(self.field, max_len))
         self.work = torch.empty(ws // 8, dtype=torch.int64, device=self.dev) if ws else None
 
@@ -288,6 +217,18 @@ class _DevicePoly:
         _check(_native.lib().gmsm_fr_poly_lincomb_device(self.field, ptrs, ln.ctypes.data, sc.ctypes.data, st.ctypes.data, off.ctypes.data,
                                                           k, d_out.data_ptr(), out_len, 1 if accumulate else 0, self.stream))
 
+    def permutation_accumulate(self, d_t1, d_t2, n: int, eps: np.ndarray, d_z):
+        """d_z = the accumulation polynomial Z of permutation.Prove in the bit-reversed Lagrange layout (n <= max_len)"""
+        _check(_native.lib().gmsm_fr_permutation_accumulate_device(self.field, d_t1.data_ptr(), d_t2.data_ptr(), n, eps.ctypes.data,
+                                                                   d_z.data_ptr(), None if self.work is None else self.work.data_ptr(),
+                                                                   self.stream))
+
+    def permutation_numerator(self, domain, d_lt1, d_lt2, d_lz, eps: np.ndarray, omega: np.ndarray, d_out):
+        """d_out = the quotient numerator of permutation.Prove on the coset of `domain` (an fft.Domain of this field)"""
+        _check(_native.lib().gmsm_fft_permutation_numerator_device(domain._h, d_lt1.data_ptr(), d_lt2.data_ptr(), d_lz.data_ptr(),
+                                                                   domain.Cardinality, eps.ctypes.data, omega.ctypes.data,
+                                                                   d_out.data_ptr(), self.stream))
+
 
 @dataclass
 class OpeningProof:
@@ -306,12 +247,11 @@ def Open(p, point: np.ndarray, pk: ProvingKey) -> OpeningProof:
     if pk.device >= 0:
         n = _poly_len(p, cp.fr_words)
         # n == 1: Commit of the empty quotient errors in the reference (kzg.go:160-162): a constant polynomial cannot be opened
-        if n <= 1 or n > pk.G1.shape[0]:
-            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        _check_size(n, 2, pk.G1.shape[0])
         import torch
 
         with torch.cuda.device(pk.device):
-            dp = _DevicePoly(pk, n)
+            dp = _DevicePoly(pk.curve, pk.device, n)
             d_f = _device_poly(p, cp.fr_words, pk.device)
             d_h, d_fa = dp.empty(n - 1), dp.empty(1)
             dp.div(d_f, n, _reduced(point, r), d_h, d_fa)
@@ -319,18 +259,14 @@ def Open(p, point: np.ndarray, pk: ProvingKey) -> OpeningProof:
             fa = d_fa.cpu().numpy().view(np.uint64)
         return OpeningProof(H=_digest(jac, pk.words), ClaimedValue=fa.copy())
     p = _host_poly(p, cp.fr_words)
-    if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
-        raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+    _check_size(p.shape[0], 1, pk.G1.shape[0])
     coeffs = _fr_decode(p, r)
     a = _fr_decode(point, r)[0]
     fa = _eval(coeffs, a, r)
     h = _divide_by_x_minus_a(coeffs, fa, a, r)
-    w = pk.words
-    # Commit(h, pk) errors on an empty h in the reference (kzg.go:160-162): a constant polynomial cannot be opened
-    H = Commit(_fr_encode(h, r), pk) if h else None
-    if H is None:
-        raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
-    return OpeningProof(H=H.reshape(w), ClaimedValue=_fr_encode([fa], r)[0])
+    # Commit(h, pk) errors on an empty h as in the reference (kzg.go:160-162): a constant polynomial cannot be opened
+    H = Commit(_fr_encode(h, r), pk)
+    return OpeningProof(H=H.reshape(pk.words), ClaimedValue=_fr_encode([fa], r)[0])
 
 
 def Commit(p, pk: ProvingKey, *nbTasks: int) -> np.ndarray:
@@ -340,17 +276,15 @@ def Commit(p, pk: ProvingKey, *nbTasks: int) -> np.ndarray:
     cfg = MultiExpConfig(NbTasks=nbTasks[0] if nbTasks else 0)
     if _is_device(p) and pk.device >= 0:
         n = _poly_len(p, words)
-        if n == 0 or n > pk.G1.shape[0]:
-            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        _check_size(n, 1, pk.G1.shape[0])
         import torch
 
         with torch.cuda.device(pk.device):
             d = _device_poly(p, words, pk.device)
-            jac = pk._bases.MultiExpDevice(d, n, cfg, stream=torch.cuda.current_stream(d.device).cuda_stream)
+            jac = pk._bases.MultiExpDevice(d, n, cfg, stream=_stream(d.device))
         return _digest(jac, pk.words)
     p = _host_poly(p, words)
-    if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
-        raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+    _check_size(p.shape[0], 1, pk.G1.shape[0])
     return _digest(pk._bases.MultiExp(p, cfg), pk.words)
 
 
@@ -493,27 +427,21 @@ class BatchOpeningProof:
     ClaimedValues: np.ndarray
 
 
-def _fr_marshal(limbs, r: int) -> bytes:
-    """fr.Element.Marshal (fr/element.go:868-871): fr.Bytes (8 * fr.Limbs) bytes big-endian, canonical value"""
-    return _fr_decode(np.asarray(limbs, dtype=np.uint64), r)[0].to_bytes(8 * _limbs(r), "big")
-
-
 def derive_gamma(point, digests, claimed_values, hf, curve: str, *data_transcript: bytes) -> int:
     """deriveGamma (kzg.go:531-563) over fiatshamir.Transcript (fiat-shamir/transcript.go:61-131) with the single challenge
     "gamma": H("gamma" || point || digests (RawBytes) || claimed values || extra data), read big-endian and reduced mod r
     (fr.SetBytes, fr/element.go:880-903).  `hf` is a hashlib constructor (e.g. hashlib.sha256)."""
-    c = curve.split("_")[0]
-    cp = CURVE_PARAMS[c]
+    cp = _params(curve)
     r = cp.r
     fs = Transcript(hf, "gamma")
     fs.Bind("gamma", _fr_marshal(point, r))
     for d in digests:
-        fs.Bind("gamma", g1_raw_bytes(d, c))
+        fs.Bind("gamma", g1_raw_bytes(d, curve))
     for v in np.ascontiguousarray(claimed_values, dtype=np.uint64).reshape(-1, cp.fr_words):
         fs.Bind("gamma", _fr_marshal(v, r))
     for b in data_transcript:
         fs.Bind("gamma", b)
-    return int.from_bytes(fs.ComputeChallenge("gamma"), "big") % r
+    return _challenge(fs, "gamma", r)
 
 
 def BatchOpenSinglePoint(polynomials, digests, point: np.ndarray, hf, pk: ProvingKey, *data_transcript: bytes) -> BatchOpeningProof:
@@ -523,21 +451,19 @@ def BatchOpenSinglePoint(polynomials, digests, point: np.ndarray, hf, pk: Provin
     the transcript, the folded polynomial and its quotient never leave the device."""
     if len(digests) != len(polynomials):
         raise ErrInvalidNbDigests("number of digests is not the same as the number of polynomials")
-    c = pk.curve.split("_")[0]
-    cp = CURVE_PARAMS[c]
+    cp = _params(pk.curve)
     r = cp.r
     if pk.device >= 0:
         return _batch_open_device(polynomials, digests, point, hf, pk, *data_transcript)
     polys = []
     for p in polynomials:
         p = _host_poly(p, cp.fr_words)
-        if p.shape[0] == 0 or p.shape[0] > pk.G1.shape[0]:
-            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        _check_size(p.shape[0], 1, pk.G1.shape[0])
         polys.append(_fr_decode(p, r))
     a = _fr_decode(point, r)[0]
     claimed = [_eval(f, a, r) for f in polys]
     claimed_limbs = _fr_encode(claimed, r)
-    gamma = derive_gamma(point, digests, claimed_limbs, hf, c, *data_transcript)
+    gamma = derive_gamma(point, digests, claimed_limbs, hf, pk.curve, *data_transcript)
     folded_eval = claimed[-1]
     for v in reversed(claimed[:-1]):
         folded_eval = (folded_eval * gamma + v) % r
@@ -549,36 +475,31 @@ def BatchOpenSinglePoint(polynomials, digests, point: np.ndarray, hf, pk: Provin
         for j, v in enumerate(f):
             folded[j] = (folded[j] + v * g) % r
     h = _divide_by_x_minus_a(folded, folded_eval, a, r)
-    if not h:
-        raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
-    H = Commit(_fr_encode(h, r), pk)
+    H = Commit(_fr_encode(h, r), pk)          # errors on an empty h, as in the reference
     return BatchOpeningProof(H=H.reshape(pk.words), ClaimedValues=claimed_limbs)
 
 
 def _batch_open_device(polynomials, digests, point, hf, pk: ProvingKey, *data_transcript: bytes) -> BatchOpeningProof:
     import torch
 
-    c = pk.curve.split("_")[0]
-    cp = CURVE_PARAMS[c]
+    cp = _params(pk.curve)
     r, w = cp.r, cp.fr_words
     lens = []
     for p in polynomials:
         n = _poly_len(p, w)
-        if n == 0 or n > pk.G1.shape[0]:
-            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        _check_size(n, 1, pk.G1.shape[0])
         lens.append(n)
     largest = max(lens)
     a = _reduced(point, r)
     with torch.cuda.device(pk.device):
-        dp = _DevicePoly(pk, largest)
+        dp = _DevicePoly(pk.curve, pk.device, largest)
         d_polys = [_device_poly(p, w, pk.device) for p in polynomials]
         d_claimed = dp.empty(len(lens))
         for i, (d_f, n) in enumerate(zip(d_polys, lens)):
             dp.div(d_f, n, a, None, d_claimed[i * w:(i + 1) * w])
         claimed_limbs = d_claimed.cpu().numpy().view(np.uint64).reshape(-1, w).copy()
-        gamma = derive_gamma(point, digests, claimed_limbs, hf, c, *data_transcript)
-        if largest == 1:        # the folded quotient is empty: Commit errors in the reference
-            raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
+        gamma = derive_gamma(point, digests, claimed_limbs, hf, pk.curve, *data_transcript)
+        _check_size(largest, 2, pk.G1.shape[0])     # the folded quotient is empty: Commit errors in the reference
         d_fold = dp.empty(largest)
         dp.fold(d_polys, lens, _fr_encode([gamma], r)[0], d_fold, largest)
         d_h, d_fa = dp.empty(largest - 1), dp.empty(1)
@@ -592,19 +513,18 @@ def FoldProof(digests, proof: BatchOpeningProof, point: np.ndarray, hf, curve: s
     host, the digests with one MultiExp (`fold`, kzg.go:506-528 -- the reference calls MultiExp for it too)."""
     from .multiexp import curve_package
 
-    c = curve.split("_")[0]
-    cp = CURVE_PARAMS[c]
+    cp = _params(curve)
     claimed = np.ascontiguousarray(proof.ClaimedValues, dtype=np.uint64).reshape(-1, cp.fr_words)
     if len(digests) != claimed.shape[0]:
         raise ErrInvalidNbDigests("number of digests is not the same as the number of polynomials")
     r = cp.r
-    gamma = derive_gamma(point, digests, claimed, hf, c, *data_transcript)
+    gamma = derive_gamma(point, digests, claimed, hf, curve, *data_transcript)
     gam = [1]
     for _ in range(1, len(digests)):
         gam.append(gam[-1] * gamma % r)
     vals = _fr_decode(claimed, r)
     folded_eval = sum(v * g for v, g in zip(vals, gam)) % r
-    aff_cls = curve_package(c)[0]
+    aff_cls = curve_package(_curve(curve))[0]
     pts = np.ascontiguousarray(np.stack([np.asarray(d, dtype=np.uint64).reshape(-1) for d in digests]))
     folded_digest = aff_cls().MultiExp(pts, _fr_encode(gam, r), MultiExpConfig()).limbs
     return OpeningProof(H=np.array(proof.H, dtype=np.uint64), ClaimedValue=_fr_encode([folded_eval], r)[0]), folded_digest
@@ -613,18 +533,14 @@ def FoldProof(digests, proof: BatchOpeningProof, point: np.ndarray, hf, curve: s
 def decode_g1_points(curve: str, data: bytes, n: int, raw: bool = False, check_on_curve: bool = True) -> np.ndarray:
     """bulk G1Affine.SetBytes on the GPU (gmsm_g1_decode, csrc/decode.cu): n points of a homogeneous stream -> (n, words) uint64
     in Go memory layout.  Raises MultiExpError with the reference's message and the index of the first invalid point."""
-    from . import _native
-
-    cname = curve + "_g1" if not curve.endswith("_g1") else curve
-    words = 2 * _words(CURVES[cname])
+    g = GROUPS[_g1_name(curve)]
+    words = 2 * g.words
     per = 8 * words if raw else 4 * words
     if len(data) < n * per:
         raise EOFError("short buffer")      # io.ErrShortBuffer
     buf = np.frombuffer(data, dtype=np.uint8, count=n * per)
     out = np.zeros((n, words), dtype=np.uint64)
-    rc = _native.lib().gmsm_g1_decode(CURVES[cname], buf.ctypes.data, n, 1 if raw else 0, 1 if check_on_curve else 0, out.ctypes.data)
-    if rc != 0:
-        raise MultiExpError(_native.last_error())
+    _check(_native.lib().gmsm_g1_decode(g.id, buf.ctypes.data, n, 1 if raw else 0, 1 if check_on_curve else 0, out.ctypes.data))
     return out
 
 
@@ -639,7 +555,7 @@ def ToLagrangeG1(coeffs, curve: str, device: int = 0):
     if cname not in CURVES:
         raise MultiExpError("unknown curve %r" % curve)
     cid = CURVES[cname]
-    words = 2 * _words(cid)
+    words = 2 * GROUPS[cname].words
     L = _native.lib()
     if _is_device(coeffs):
         import torch
@@ -651,8 +567,7 @@ def ToLagrangeG1(coeffs, curve: str, device: int = 0):
         with torch.cuda.device(coeffs.device):
             ws = int(L.gmsm_g1_to_lagrange_workspace_bytes(cid, n))
             work = torch.empty(max(ws // 8, 1), dtype=torch.int64, device=coeffs.device)
-            st = torch.cuda.current_stream(coeffs.device).cuda_stream
-            _check(L.gmsm_g1_to_lagrange_device(cid, coeffs.data_ptr(), n, out.data_ptr(), work.data_ptr(), st))
+            _check(L.gmsm_g1_to_lagrange_device(cid, coeffs.data_ptr(), n, out.data_ptr(), work.data_ptr(), _stream(coeffs.device)))
         return out
     pts = np.ascontiguousarray(coeffs, dtype=np.uint64).reshape(-1, words)
     out = np.empty_like(pts)
@@ -665,20 +580,15 @@ def CommitLagrange(evals, pk: ProvingKey, domain) -> np.ndarray:
     once, FFTInverse(DIF) + BitReverse (fft.go:111-190, bitreverse.go:17-42) run there and their output -- the coefficients,
     still in device memory, Montgomery form -- feeds the MultiExp directly (gmsm_bases_multiexp_device): the canonical-form
     coefficients never visit the host.  Equals Commit(FFTInverse(evals), pk)."""
-    import torch
-
     from .fft import DIF
 
-    ev = np.ascontiguousarray(evals, dtype=np.uint64).reshape(-1, _params(pk.curve).fr_words)
+    words = _params(pk.curve).fr_words
+    ev = np.ascontiguousarray(evals, dtype=np.uint64).reshape(-1, words)      # host evaluations only
     if ev.shape[0] != domain.Cardinality:
         raise MultiExpError("len(a) must equal the domain cardinality")
-    if ev.shape[0] == 0 or ev.shape[0] > pk.G1.shape[0]:
-        raise ErrInvalidPolynomialSize("invalid polynomial size (larger than SRS or == 0)")
-    dev = torch.device("cuda", domain.device)
-    d = torch.from_numpy(ev.view(np.int64).reshape(-1).copy()).to(dev)
-    st = torch.cuda.current_stream(dev).cuda_stream
+    _check_size(ev.shape[0], 1, pk.G1.shape[0])
+    d = _device_poly(ev, words, domain.device)          # a fresh upload: transformed in place below
+    st = _stream(domain.device)
     domain.fft_device(d, True, DIF, False, st)          # natural in, bit-reversed out
     domain.bit_reverse_device(d, st)
-    jac = pk._bases.MultiExpDevice(d, ev.shape[0], stream=st)
-    w = pk.words
-    return jac[:w].copy() if jac[w:].any() else np.zeros(w, dtype=np.uint64)
+    return _digest(pk._bases.MultiExpDevice(d, ev.shape[0], stream=st), pk.words)

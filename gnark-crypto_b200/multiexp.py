@@ -21,18 +21,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _native
-
-CURVES = {"bn254_g1": 0, "bn254_g2": 1, "bls12381_g1": 2, "bls12381_g2": 3, "bls12377_g1": 4, "bls12377_g2": 5,
-          # N4 remainder: ecc/secp256k1/multiexp.go:32 ; ecc/bw6-761/multiexp.go:32, :306 (G2 of bw6-761 is over Fp too)
-          "secp256k1_g1": 6, "bw6761_g1": 7, "bw6761_g2": 8,
-          # ecc/bls24-315/multiexp.go:32, ecc/bls24-317/multiexp.go:32 (G1 only: their G2 is over Fp4) ; ecc/bw6-633/multiexp.go:32, :304
-          "bls24315_g1": 9, "bls24317_g1": 10, "bw6633_g1": 11, "bw6633_g2": 12}
-# u64 words: (coordinate limbs L, coordinates per point-coordinate: 1 = Fp, 2 = Fp2)
-_SHAPE = {0: (4, 1), 1: (4, 2), 2: (6, 1), 3: (6, 2), 4: (6, 1), 5: (6, 2), 6: (4, 1), 7: (12, 1), 8: (12, 1), 9: (5, 1), 10: (5, 1),
-          11: (10, 1), 12: (10, 1)}
-# fr.Limbs / fr.Bits of each curve id: a scalar is SCALAR_WORDS x uint64 in Montgomery form
-SCALAR_WORDS = {0: 4, 1: 4, 2: 4, 3: 4, 4: 4, 5: 4, 6: 4, 7: 6, 8: 6, 9: 4, 10: 4, 11: 5, 12: 5}
-SCALAR_BITS = {0: 254, 1: 254, 2: 255, 3: 255, 4: 253, 5: 253, 6: 256, 7: 377, 8: 377, 9: 253, 10: 255, 11: 315, 12: 315}
+from .curves import CURVES, GROUPS
 
 
 class MultiExpError(Exception):
@@ -46,14 +35,16 @@ class MultiExpConfig:
     NbTasks: int = 0
 
 
-def _words(cid):
-    L, e = _SHAPE[cid]
-    return L * e
-
-
 def _check(rc):
     if rc != 0:
         raise MultiExpError(_native.last_error())
+
+
+def _handle(h):
+    """a handle the library returned; NULL is its error"""
+    if not h:
+        raise MultiExpError(_native.last_error())
+    return h
 
 
 def _as_u64(a, cols, what):
@@ -68,7 +59,7 @@ def _as_u64(a, cols, what):
 
 
 class _Point:
-    CURVE_ID = None  # set by curve_package()
+    GROUP = None  # set by curve_package()
     WORDS = 0
 
     def __init__(self, limbs=None):
@@ -85,15 +76,15 @@ class _JacBase(_Point):
     def MultiExp(self, points, scalars, config: MultiExpConfig = None):
         """(*G1Jac).MultiExp / (*G2Jac).MultiExp -- one-shot, host buffers (gmsm_multiexp)."""
         config = config or MultiExpConfig()
-        cid = self.CURVE_ID
-        w = _words(cid)
+        g = self.GROUP
+        w = g.words
         points = _as_u64(points, 2 * w, "points")
-        scalars = _as_u64(scalars, SCALAR_WORDS[cid], "scalars")
+        scalars = _as_u64(scalars, g.scalar_words, "scalars")
         if points.shape[0] != scalars.shape[0]:
             raise MultiExpError("len(points) != len(scalars)")  # multiexp.go:61-64
         out = np.zeros(3 * w, dtype=np.uint64)
         L = _native.lib()
-        rc = L.gmsm_multiexp(cid, points.ctypes.data, scalars.ctypes.data, points.shape[0], int(config.NbTasks), out.ctypes.data)
+        rc = L.gmsm_multiexp(g.id, points.ctypes.data, scalars.ctypes.data, points.shape[0], int(config.NbTasks), out.ctypes.data)
         _check(rc)
         self.limbs = out
         return self
@@ -151,10 +142,9 @@ def curve_package(curve: str):
         if "%s_%s" % (curve, grp) not in CURVES:   # secp256k1: G1 only
             out += [None, None]
             continue
-        cid = CURVES["%s_%s" % (curve, grp)]
-        w = _words(cid)
-        jac = type("%s_%sJac" % (curve, grp.upper()), (_JacBase,), {"CURVE_ID": cid, "WORDS": 3 * w})
-        aff = type("%s_%sAffine" % (curve, grp.upper()), (_AffBase,), {"CURVE_ID": cid, "WORDS": 2 * w, "JAC": jac})
+        g = GROUPS["%s_%s" % (curve, grp)]
+        jac = type("%s_%sJac" % (curve, grp.upper()), (_JacBase,), {"GROUP": g, "WORDS": 3 * g.words})
+        aff = type("%s_%sAffine" % (curve, grp.upper()), (_AffBase,), {"GROUP": g, "WORDS": 2 * g.words, "JAC": jac})
         out += [aff, jac]
     return tuple(out)
 
@@ -168,17 +158,15 @@ class ResidentBases:
 
     def __init__(self, curve: str, points, device: int = 0):
         self.cid = CURVES[curve]
-        self.w = _words(self.cid)
+        self.w = GROUPS[curve].words
+        self.sw = GROUPS[curve].scalar_words
         points = _as_u64(points, 2 * self.w, "points")
         self.n = points.shape[0]
-        L = _native.lib()
-        self._h = L.gmsm_bases_upload(self.cid, points.ctypes.data, self.n, device)
-        if not self._h:
-            raise MultiExpError(_native.last_error())
+        self._h = _handle(_native.lib().gmsm_bases_upload(self.cid, points.ctypes.data, self.n, device))
 
     def MultiExp(self, scalars, config: MultiExpConfig = None, offset: int = 0):
         config = config or MultiExpConfig()
-        scalars = _as_u64(scalars, SCALAR_WORDS[self.cid], "scalars")
+        scalars = _as_u64(scalars, self.sw, "scalars")
         out = np.zeros(3 * self.w, dtype=np.uint64)
         rc = _native.lib().gmsm_bases_multiexp(self._h, offset, scalars.ctypes.data, scalars.shape[0], int(config.NbTasks), out.ctypes.data)
         _check(rc)
@@ -189,7 +177,7 @@ class ResidentBases:
         fft.Domain.fft_device): nothing but the 96..288-byte result crosses PCIe"""
         config = config or MultiExpConfig()
         if n is None:
-            n = d_scalars.numel() // SCALAR_WORDS[self.cid]
+            n = d_scalars.numel() // self.sw
         out = np.zeros(3 * self.w, dtype=np.uint64)
         rc = _native.lib().gmsm_bases_multiexp_device(self._h, offset, d_scalars.data_ptr(), n, int(config.NbTasks), out.ctypes.data, stream)
         _check(rc)
@@ -223,14 +211,12 @@ class Engine:
         self.torch = torch
         self.curve = curve
         self.cid = CURVES[curve]
-        self.w = _words(self.cid)
-        self.sw = SCALAR_WORDS[self.cid]       # u64 words per scalar
+        self.w = GROUPS[curve].words
+        self.sw = GROUPS[curve].scalar_words   # u64 words per scalar
         self.device = device
         self.tables = tables
         L = _native.lib()
-        self._h = (L.gmsm_ctx_create_tables if tables else L.gmsm_ctx_create)(self.cid, max_n, c, device)
-        if not self._h:
-            raise MultiExpError(_native.last_error())
+        self._h = _handle((L.gmsm_ctx_create_tables if tables else L.gmsm_ctx_create)(self.cid, max_n, c, device))
         self.c = L.gmsm_ctx_window_bits(self._h)
         self.nwin = L.gmsm_ctx_num_windows(self._h)
         self.workspace_bytes = L.gmsm_ctx_workspace_bytes(self._h)
@@ -326,12 +312,11 @@ class Engine:
 def BatchScalarMultiplication(curve: str, base, scalars) -> np.ndarray:
     """BatchScalarMultiplicationG1 / G2 (ecc/bn254/g1.go:1039-1118, g2.go:1001+): multiplies the same
     base by all scalars; returns the points in affine coordinates, shape (n, 2*words) uint64."""
-    cid = CURVES[curve]
-    w = _words(cid)
-    base = np.ascontiguousarray(base, dtype=np.uint64).reshape(2 * w)
-    scalars = _as_u64(scalars, SCALAR_WORDS[cid], "scalars")
-    out = np.zeros((scalars.shape[0], 2 * w), dtype=np.uint64)
-    rc = _native.lib().gmsm_batch_scalar_mul(cid, base.ctypes.data, scalars.ctypes.data, scalars.shape[0], out.ctypes.data)
+    g = GROUPS[curve]
+    base = np.ascontiguousarray(base, dtype=np.uint64).reshape(2 * g.words)
+    scalars = _as_u64(scalars, g.scalar_words, "scalars")
+    out = np.zeros((scalars.shape[0], 2 * g.words), dtype=np.uint64)
+    rc = _native.lib().gmsm_batch_scalar_mul(g.id, base.ctypes.data, scalars.ctypes.data, scalars.shape[0], out.ctypes.data)
     _check(rc)
     return out
 
@@ -348,11 +333,11 @@ def test_op(curve: str, op: int, a: np.ndarray, b: np.ndarray, out_words: int) -
 
 
 def test_digits(curve: str, c: int, scalars: np.ndarray) -> np.ndarray:
-    scalars = _as_u64(scalars, SCALAR_WORDS[CURVES[curve]], "scalars")
+    g = GROUPS[curve]
+    scalars = _as_u64(scalars, g.scalar_words, "scalars")
     n = scalars.shape[0]
-    bits = SCALAR_BITS[CURVES[curve]]
-    W = (bits + c - 1) // c
+    W = (g.scalar_bits + c - 1) // c
     out = np.zeros((W, n), dtype=np.uint32)
-    rc = _native.lib().gmsm_test_digits(CURVES[curve], c, scalars.ctypes.data, n, out.ctypes.data)
+    rc = _native.lib().gmsm_test_digits(g.id, c, scalars.ctypes.data, n, out.ctypes.data)
     _check(rc)
     return out

@@ -15,10 +15,11 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from . import _native, fft, kzg
+from . import fft, kzg
+from .curves import _challenge, _curve, _fr_decode, _fr_encode, _params
 from .fft import DIF, DIT
-from .kzg import _fr_decode, _fr_encode, g1_raw_bytes
-from .multiexp import MultiExpError, _check
+from .kzg import g1_raw_bytes
+from .multiexp import MultiExpError
 from .transcript import Transcript
 
 
@@ -50,43 +51,34 @@ def Prove(pk: kzg.ProvingKey, t1, t2) -> Proof:
     device for a single-device key), left unmodified.  The work is ordered on the current stream of the device."""
     import torch
 
-    cp = kzg._params(pk.curve)
-    r, w = cp.r, cp.fr_words
+    w = _params(pk.curve).fr_words
     n = kzg._poly_len(t1, w)
     if n != kzg._poly_len(t2, w):
         raise ErrIncompatibleSize("t1 and t2 should be of the same size")
     # NewDomain(n).Cardinality != n (NextPowerOfTwo(0) = 1): refused before a domain is built
     if n == 0 or n & (n - 1):
         raise ErrSize("t1 and t2 should be of size a power of 2")
-    curve = pk.curve.split("_")[0]
-    dev_id = pk.device if pk.device >= 0 else torch.cuda.current_device()
-    d = fft.NewDomain(curve, n, device=dev_id)
+    curve = _curve(pk.curve)
+    dev = pk.device if pk.device >= 0 else torch.cuda.current_device()
+    d = fft.NewDomain(curve, n, device=dev)
     try:
-        with torch.cuda.device(dev_id):
-            return _prove(pk, d, t1, t2, n, curve, torch.device("cuda", dev_id))
+        with torch.cuda.device(dev):
+            return _prove(pk, d, t1, t2, n, curve, dev)
     finally:
         d.close()
 
 
-def _challenge(fs: Transcript, name: str, r: int) -> int:
-    """fr.Element.SetBytes of the raw challenge: big-endian, reduced mod r"""
-    return int.from_bytes(fs.ComputeChallenge(name), "big") % r
-
-
 def _prove(pk, d, t1, t2, n, curve, dev):
-    import torch
-
-    cp = kzg._params(curve)
+    cp = _params(curve)
     r, w = cp.r, cp.fr_words
-    field = fft._FIELDS[curve]
-    L = _native.lib()
-    st = torch.cuda.current_stream(dev).cuda_stream
+    dp = kzg._DevicePoly(curve, dev, n)
+    st = dp.stream
     sharded = pk.device < 0
 
     def commit(p):
-        return kzg.Commit(_host(p, w) if sharded else p, pk)
+        return kzg.Commit(kzg._host_poly(p, w) if sharded else p, pk)
 
-    d_t1, d_t2 = (kzg._device_poly(t, w, dev.index) for t in (t1, t2))   # device tensors in place, host arrays uploaded once
+    d_t1, d_t2 = (kzg._device_poly(t, w, dev) for t in (t1, t2))   # device tensors in place, host arrays uploaded once
     ct1, ct2 = d_t1.clone(), d_t2.clone()
     for ct in (ct1, ct2):                                   # coefficients: FFTInverse(DIF) + BitReverse
         d.fft_device(ct, True, DIF, False, st)
@@ -97,11 +89,8 @@ def _prove(pk, d, t1, t2, n, curve, dev):
         fs.Bind("epsilon", g1_raw_bytes(p, curve))
     eps = _fr_encode([_challenge(fs, "epsilon", r)], r)[0]
     # Z in the bit-reversed Lagrange layout, then its coefficients by FFTInverse(DIT)
-    cz = torch.empty(n * w, dtype=torch.int64, device=dev)
-    ws = int(L.gmsm_fr_permutation_workspace_bytes(field, n))
-    work = torch.empty(ws // 8, dtype=torch.int64, device=dev) if ws else None
-    _check(L.gmsm_fr_permutation_accumulate_device(field, d_t1.data_ptr(), d_t2.data_ptr(), n, eps.ctypes.data,
-                                                   cz.data_ptr(), None if work is None else work.data_ptr(), st))
+    cz = dp.empty(n)
+    dp.permutation_accumulate(d_t1, d_t2, n, eps, cz)
     d.fft_device(cz, True, DIT, False, st)
     Z = commit(cz)
     # the three coset evaluations (bit-reversed), the numerator, and the quotient's coefficients
@@ -110,9 +99,8 @@ def _prove(pk, d, t1, t2, n, curve, dev):
         d.fft_device(v, False, DIF, True, st)
     fs.Bind("omega", g1_raw_bytes(Z, curve))
     omega = _fr_encode([_challenge(fs, "omega", r)], r)[0]
-    qv = torch.empty(n * w, dtype=torch.int64, device=dev)
-    _check(L.gmsm_fft_permutation_numerator_device(d._h, lt1.data_ptr(), lt2.data_ptr(), lz.data_ptr(), n, eps.ctypes.data,
-                                                   omega.ctypes.data, qv.data_ptr(), st))
+    qv = dp.empty(n)
+    dp.permutation_numerator(d, lt1, lt2, lz, eps, omega, qv)
     del lz, lt1, lt2
     d.fft_device(qv, True, DIT, True, st)
     Q = commit(qv)
@@ -120,13 +108,9 @@ def _prove(pk, d, t1, t2, n, curve, dev):
     eta = _challenge(fs, "eta", r)
     polys = [ct1, ct2, cz, qv]
     if sharded:
-        polys = [_host(p, w) for p in polys]
+        polys = [kzg._host_poly(p, w) for p in polys]
     batched = kzg.BatchOpenSinglePoint(polys, [T1, T2, Z, Q], _fr_encode([eta], r)[0], hashlib.sha256, pk)
     gen = _fr_decode(d.Generator, r)[0]
     shifted = kzg.Open(polys[2], _fr_encode([eta * gen % r], r)[0], pk)
     return Proof(size=n, g=d.Generator.copy(), t1=T1, t2=T2, z=Z, q=Q, batchedProof=batched, shiftedProof=shifted)
-
-
-def _host(p, w):
-    return kzg._host_poly(p, w)
 

@@ -21,11 +21,10 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import kzg
-from .kzg import ErrInvalidPolynomialSize, _fr_decode, _fr_encode, g1_raw_bytes
+from .curves import _challenge, _fr_decode, _fr_encode, _limbs, _params
+from .kzg import _check_size, g1_raw_bytes
 from .multiexp import MultiExpError
 from .transcript import Transcript
-
-_SIZE_ERR = "invalid polynomial size (larger than SRS or == 0)"
 
 
 class ErrInvalidNumberOfPoints(MultiExpError):
@@ -56,7 +55,7 @@ def BatchOpen(polynomials, digests, points, hf, pk: kzg.ProvingKey, *dataTranscr
         raise ErrInvalidNumberOfDigests("number of digests should be equal to the number of polynomials")
     if not polynomials:
         raise ValueError("shplonk.BatchOpen needs at least one polynomial")
-    cp = kzg._params(pk.curve)
+    cp = _params(pk.curve)
     r, w = cp.r, cp.fr_words
     pts = [_decode_points(S, r) for S in points]
     if pk.device < 0:
@@ -68,30 +67,24 @@ def BatchOpen(polynomials, digests, points, hf, pk: kzg.ProvingKey, *dataTranscr
 
 
 def _decode_points(S, r: int) -> list:
-    return _fr_decode(np.asarray(S, dtype=np.uint64).reshape(-1, kzg._limbs(r)), r)
+    return _fr_decode(np.asarray(S, dtype=np.uint64).reshape(-1, _limbs(r)), r)
 
 
 def _host_commit(pk: kzg.ProvingKey):
-    r = kzg._params(pk.curve).r
+    r = _params(pk.curve).r
     return lambda coeffs: kzg.Commit(_fr_encode(coeffs, r), pk)
-
-
-def _challenge(fs: Transcript, name: str, r: int) -> int:
-    """fr.Element.SetBytes of the raw challenge: big-endian, reduced mod r"""
-    return int.from_bytes(fs.ComputeChallenge(name), "big") % r
 
 
 def _transcript(hf, ext_points, digests, curve: str, data) -> Transcript:
     """deriveChallenge("gamma", ...) (shplonk.go:278-308) up to the challenge: every point (fr.Marshal), every digest (RawBytes),
     the data transcript"""
-    c = curve.split("_")[0]
-    nb = kzg._params(c).fr_bytes
+    nb = _params(curve).fr_bytes
     fs = Transcript(hf, "gamma", "z")
     for S in ext_points:
         for x in S:
             fs.Bind("gamma", x.to_bytes(nb, "big"))
     for d in digests:
-        fs.Bind("gamma", g1_raw_bytes(d, c))
+        fs.Bind("gamma", g1_raw_bytes(d, curve))
     for b in data:
         fs.Bind("gamma", b)
     return fs
@@ -111,20 +104,20 @@ def open_packs(packs, base_points, ts, ext_points, digests, hf, pk: kzg.ProvingK
     the s^t_j of base_points[j]), all values as Python ints."""
     import torch
 
-    cp = kzg._params(pk.curve)
+    cp = _params(pk.curve)
     r, w = cp.r, cp.fr_words
     lens = [[kzg._poly_len(p, w) for p in pack] for pack in packs]
     max_size, nb_points = _sizes([t * max(ln, default=0) for t, ln in zip(ts, lens)], ext_points)
     n_srs = pk.G1.shape[0]
     # the reference's Commit checks: W has maxSizePolys coefficients, W' has maxSizePolys + |T| - 1 (zero past maxSizePolys - 1)
-    if max_size > n_srs or not 0 < max_size + nb_points - 1 <= n_srs:
-        raise ErrInvalidPolynomialSize(_SIZE_ERR)
+    _check_size(max_size, 0, n_srs)
+    _check_size(max_size + nb_points - 1, 1, n_srs)
     fs = _transcript(hf, ext_points, digests, pk.curve, data)
     gamma = _challenge(fs, "gamma", r)
     enc = lambda v: _fr_encode([v % r], r)[0]          # noqa: E731
     ys = [[pow(s, t, r) for s in S] for S, t in zip(base_points, ts)]
     with torch.cuda.device(pk.device):
-        dp = kzg._DevicePoly(pk, max_size)
+        dp = kzg._DevicePoly(pk.curve, pk.device, max_size)
         d_in = [[kzg._device_poly(p, w, pk.device) if n else None for p, n in zip(pack, ln)] for pack, ln in zip(packs, lens)]
         slots = sum(len(pack) * len(y) for pack, y in zip(packs, ys))
         d_newton = torch.zeros(max(slots, 1) * w, dtype=torch.int64, device=dp.dev)
@@ -151,7 +144,7 @@ def open_packs(packs, base_points, ts, ext_points, digests, hf, pk: kzg.ProvingK
         else:
             d_W.zero_()
         W = kzg._digest(pk._bases.MultiExpDevice(d_W, max_size, stream=dp.stream), pk.words)
-        fs.Bind("z", g1_raw_bytes(W, pk.curve.split("_")[0]))
+        fs.Bind("z", g1_raw_bytes(W, pk.curve))
         z = _challenge(fs, "z", r)
         # L = sum_j c_j F_j - Z_T(z) W, c_j = gamma^j Z_{T\S_j}(z); W' = quotient of L by (X - z)
         zdiff = [[(z - x) % r for x in S] for S in ext_points]
@@ -282,7 +275,7 @@ def _div(f, g, r):
 def batch_open_host(polys, points, digests, hf, curve: str, commit, *data):
     """BatchOpen (shplonk.go:44-172) on Python ints: polys[i] and points[i] lists of ints; commit(coeffs) -> digest limbs (kzg.Commit
     and its errors).  Returns (W, W', claimed values, w, w') with w and w' the committed coefficient lists."""
-    r = kzg._params(curve).r
+    r = _params(curve).r
     fs = _transcript(hf, points, digests, curve, data)
     gamma = _challenge(fs, "gamma", r)
     max_size, nb_points = _sizes([len(p) for p in polys], points)
@@ -303,7 +296,7 @@ def batch_open_host(polys, points, digests, hf, curve: str, commit, *data):
     zt = _vanishing([x for S in points for x in S], r)
     w = _div(f, zt, r)
     W = commit(w)
-    fs.Bind("z", g1_raw_bytes(W, curve.split("_")[0]))
+    fs.Bind("z", g1_raw_bytes(W, curve))
     z = _challenge(fs, "z", r)
     acc = 1
     lpoly = [0] * total

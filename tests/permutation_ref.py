@@ -14,6 +14,8 @@ from oracle import cref
 from oracle import oracle as O
 from tests import fft_more_fields as M
 
+curves = import_module("gnark-crypto_b200.curves")
+
 DIT, DIF = O.DIT, O.DIF
 
 
@@ -143,7 +145,7 @@ def _batch_open(polys, digests, eta, srs, curve):
     kzg = _kzg()
     r = srs.r
     claimed = [_ev(f, eta, r) for f in polys]
-    gamma = kzg.derive_gamma(kzg._fr_encode([eta], r)[0], digests, kzg._fr_encode(claimed, r), hashlib.sha256, curve)
+    gamma = kzg.derive_gamma(curves._fr_encode([eta], r)[0], digests, curves._fr_encode(claimed, r), hashlib.sha256, curve)
     largest = max(len(f) for f in polys)
     folded, g = [0] * largest, 1
     for f in polys:
@@ -209,8 +211,8 @@ def verify(curve, proof, alpha):
     omega = _challenge(fs, "omega", r)
     fs.Bind("eta", kzg.g1_raw_bytes(proof.q, curve))
     eta = _challenge(fs, "eta", r)
-    cl = kzg._fr_decode(proof.batchedProof.ClaimedValues, r)
-    zs = kzg._fr_decode(proof.shiftedProof.ClaimedValue, r)[0]
+    cl = curves._fr_decode(proof.batchedProof.ClaimedValues, r)
+    zs = curves._fr_decode(proof.shiftedProof.ClaimedValue, r)[0]
     # the relation at eta (:293-311)
     rhs = (pow(eta, proof.size, r) - 1) % r
     l0 = rhs * pow((eta - 1) % r, r - 2, r) % r
@@ -230,11 +232,11 @@ def verify(curve, proof, alpha):
         return not aff.any()
 
     # BatchVerifySinglePoint (kzg.go:420-470): fold the digests and values with gamma
-    gamma = kzg.derive_gamma(kzg._fr_encode([eta], r)[0], digests, proof.batchedProof.ClaimedValues, hashlib.sha256, curve)
+    gamma = kzg.derive_gamma(curves._fr_encode([eta], r)[0], digests, proof.batchedProof.ClaimedValues, hashlib.sha256, curve)
     gam = [pow(gamma, i, r) for i in range(4)]
     if not opening_holds(list(zip(digests, gam)), sum(g * v for g, v in zip(gam, cl)) % r, eta, proof.batchedProof.H):
         return False
-    g = kzg._fr_decode(proof.g, r)[0]
+    g = curves._fr_decode(proof.g, r)[0]
     if not opening_holds([(proof.z, 1)], zs, eta * g % r, proof.shiftedProof.H):
         return False
     # the generator's order (:333-344)

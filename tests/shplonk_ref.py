@@ -13,6 +13,8 @@ import numpy as np
 from oracle import cref
 from oracle import oracle as O
 
+curves = import_module("gnark-crypto_b200.curves")
+
 
 def _mods():
     return import_module("gnark-crypto_b200.kzg"), import_module("gnark-crypto_b200.shplonk"), import_module("gnark-crypto_b200.fflonk")
@@ -43,7 +45,7 @@ def identity_open(packs, base_points, ts, ext_points, digests, hf, curve, commit
     r = kzg.CURVE_PARAMS[curve].r
     max_size, nb_points = shplonk._sizes([t * max((len(p) for p in pack), default=0) for pack, t in zip(packs, ts)], ext_points)
     fs = shplonk._transcript(hf, ext_points, digests, curve, data)
-    gamma = shplonk._challenge(fs, "gamma", r)
+    gamma = curves._challenge(fs, "gamma", r)
     terms, values = [], []
     for j, (pack, S, t) in enumerate(zip(packs, base_points, ts)):
         ys = [pow(s, t, r) for s in S]
@@ -69,7 +71,7 @@ def identity_open(packs, base_points, ts, ext_points, digests, hf, curve, commit
     w = _lincomb(terms, max_size, r)
     W = commit(w)
     fs.Bind("z", kzg.g1_raw_bytes(W, curve))
-    z = shplonk._challenge(fs, "z", r)
+    z = curves._challenge(fs, "z", r)
     zt_z = 1
     for S in ext_points:
         for x in S:
@@ -134,9 +136,9 @@ def verify_in_exponent(polys, points, proof_W, proof_WPrime, claimed, digests, h
     g = curve + "_g1"
     G = O.GROUPS[g]
     fs = shplonk._transcript(hf, points, digests, curve, data)
-    gamma = shplonk._challenge(fs, "gamma", r)
+    gamma = curves._challenge(fs, "gamma", r)
     fs.Bind("z", kzg.g1_raw_bytes(proof_W, curve))
-    z = shplonk._challenge(fs, "z", r)
+    z = curves._challenge(fs, "z", r)
     gen = G.encode_affine([G.gen])[0]
     acc, sum_cr, coeffs = 1, 0, []
     for i in range(len(points)):

@@ -10,6 +10,8 @@ import subprocess
 import numpy as np
 import pytest
 
+curves = importlib.import_module("gnark-crypto_b200.curves")
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "gnark-crypto_b200", "csrc")
 EMU = os.path.join(ROOT, "tests", "emu")
@@ -56,18 +58,18 @@ def _run(c, polys, scalars, strides, offsets, out_len, init=None):
     kzg = _kzg()
     r = kzg.CURVE_PARAMS[c].r
     w = kzg.CURVE_PARAMS[c].fr_words
-    enc = [kzg._fr_encode(p, r) if p else np.zeros((1, w), dtype=np.uint64) for p in polys]
-    out = kzg._fr_encode(init, r) if init is not None else np.full((out_len, w), 0xFFFFFFFFFFFFFFFF, dtype=np.uint64)
+    enc = [curves._fr_encode(p, r) if p else np.zeros((1, w), dtype=np.uint64) for p in polys]
+    out = curves._fr_encode(init, r) if init is not None else np.full((out_len, w), 0xFFFFFFFFFFFFFFFF, dtype=np.uint64)
     ptrs = (ctypes.c_void_p * len(enc))(*[e.ctypes.data for e in enc])
     ln = np.array([len(p) for p in polys], dtype=np.uint64)
     st = np.array(strides, dtype=np.uint64)
     off = np.array(offsets, dtype=np.uint64)
-    sc = kzg._fr_encode(scalars, r)
+    sc = curves._fr_encode(scalars, r)
     rc = _lib().emu_poly_lincomb(FIELDS[c], ptrs, _ptr(ln), _ptr(sc), _ptr(st), _ptr(off), ctypes.c_uint64(len(polys)), _ptr(out),
                                  ctypes.c_uint64(out_len), 1 if init is not None else 0)
     assert rc == 0
     want = lincomb_ref(polys, scalars, strides, offsets, out_len, r, init)
-    assert np.array_equal(out, kzg._fr_encode(want, r)), (len(polys), strides, offsets, out_len)
+    assert np.array_equal(out, curves._fr_encode(want, r)), (len(polys), strides, offsets, out_len)
 
 
 def cases(r, rng):

@@ -14,6 +14,8 @@ import pytest
 
 from tests import permutation_ref as ref
 
+curves = importlib.import_module("gnark-crypto_b200.curves")
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "gnark-crypto_b200", "csrc")
 EMU = os.path.join(ROOT, "tests", "emu")
@@ -49,7 +51,7 @@ def _ptr(a):
 
 def _enc(vals, c):
     kzg = _kzg()
-    return kzg._fr_encode(vals, kzg.CURVE_PARAMS[c].r)
+    return curves._fr_encode(vals, kzg.CURVE_PARAMS[c].r)
 
 
 def _check_limbs(got, want_vals, c, what):
@@ -184,7 +186,7 @@ def test_prove_argument_errors():
         curve, device = "bn254_g1", 0
         G1 = np.zeros((64, 8), dtype=np.uint64)
 
-    t = kzg._fr_encode(list(range(8)), kzg.CURVE_PARAMS["bn254"].r)
+    t = curves._fr_encode(list(range(8)), kzg.CURVE_PARAMS["bn254"].r)
     with pytest.raises(perm.ErrIncompatibleSize, match="^t1 and t2 should be of the same size$"):
         perm.Prove(NoDeviceKey(), t, t[:4])
     with pytest.raises(perm.ErrIncompatibleSize):

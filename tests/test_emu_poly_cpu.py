@@ -11,6 +11,8 @@ import subprocess
 import numpy as np
 import pytest
 
+curves = importlib.import_module("gnark-crypto_b200.curves")
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "gnark-crypto_b200", "csrc")
 EMU = os.path.join(ROOT, "tests", "emu")
@@ -49,14 +51,14 @@ def _emu_div(c, coeffs, a, shape=None, quotient=True):
     kzg = _kzg()
     r = kzg.CURVE_PARAMS[c].r
     n = len(coeffs)
-    f = kzg._fr_encode(coeffs, r)
-    av = kzg._fr_encode([a], r)
+    f = curves._fr_encode(coeffs, r)
+    av = curves._fr_encode([a], r)
     fa = np.zeros_like(av)
     h = np.zeros((max(n - 1, 1), f.shape[1]), dtype=np.uint64)
     log_l, log_b = shape or (-1, -1)
     rc = _lib().emu_poly_div(FIELDS[c], _ptr(f), ctypes.c_uint64(n), _ptr(av), _ptr(h) if quotient else None, _ptr(fa), log_l, log_b)
     assert rc == 0, "rc = %d (2: the polynomial was modified)" % rc
-    return kzg._fr_decode(fa, r)[0], (kzg._fr_decode(h[:n - 1], r) if quotient else None), fa
+    return curves._fr_decode(fa, r)[0], (curves._fr_decode(h[:n - 1], r) if quotient else None), fa
 
 
 def _check(c, coeffs, a, shape=None):
@@ -65,7 +67,7 @@ def _check(c, coeffs, a, shape=None):
     fa, h, fa_limbs = _emu_div(c, coeffs, a, shape)
     want = kzg._eval(coeffs, a, r)
     assert fa == want
-    assert np.array_equal(fa_limbs, kzg._fr_encode([want], r))      # canonical limbs, not just the same residue
+    assert np.array_equal(fa_limbs, curves._fr_encode([want], r))      # canonical limbs, not just the same residue
     assert h == kzg._divide_by_x_minus_a(coeffs, want, a, r)
     fa2, _, _ = _emu_div(c, coeffs, a, shape, quotient=False)
     assert fa2 == want
@@ -127,12 +129,12 @@ def test_fold(c):
     for lens, gamma in cases:
         polys = [[rng.randrange(r) for _ in range(m)] for m in lens]
         polys[0][0] = r - 1
-        enc = [kzg._fr_encode(p, r) for p in polys]
+        enc = [curves._fr_encode(p, r) for p in polys]
         out_len = max(lens)
         out = np.full((out_len, enc[0].shape[1]), 0xFFFFFFFFFFFFFFFF, dtype=np.uint64)     # garbage: the first launch overwrites
         ptrs = (ctypes.c_void_p * len(enc))(*[e.ctypes.data for e in enc])
         ln = np.array(lens, dtype=np.uint64)
-        g = kzg._fr_encode([gamma], r)
+        g = curves._fr_encode([gamma], r)
         rc = _lib().emu_poly_fold(FIELDS[c], ptrs, _ptr(ln), ctypes.c_uint64(len(enc)), _ptr(g), _ptr(out), ctypes.c_uint64(out_len))
         assert rc == 0
-        assert np.array_equal(out, kzg._fr_encode(_fold_ref(polys, gamma, r, out_len), r)), (lens, gamma)
+        assert np.array_equal(out, curves._fr_encode(_fold_ref(polys, gamma, r, out_len), r)), (lens, gamma)

@@ -112,7 +112,7 @@ def test_device_point_decoding_matches_host_set_bytes(curve, g):
     with pytest.raises(kzg.MultiExpError, match="point 5: invalid infinity point encoding"):
         kzg.decode_g1_points(c, bytes(bad4), n, raw=False)
     bad5 = bytearray(raw)
-    bad5[3 * 2 * nb:3 * 2 * nb + nb] = bytes([~kzg._FLAGS[c]["mask"] & 0xFF]) + b"\xff" * (nb - 1)   # x >= q, flag bits zero (uncompressed)
+    bad5[3 * 2 * nb:3 * 2 * nb + nb] = bytes([~kzg.CURVE_PARAMS[c].flags["mask"] & 0xFF]) + b"\xff" * (nb - 1)   # x >= q, flag bits zero (uncompressed)
     with pytest.raises(kzg.MultiExpError, match="point 3: invalid fp.Element encoding"):
         kzg.decode_g1_points(c, bytes(bad5), n, raw=True)
 

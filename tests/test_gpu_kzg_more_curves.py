@@ -11,12 +11,25 @@ import pytest
 from oracle import cref
 from oracle import oracle as O
 
+curves = import_module("gnark-crypto_b200.curves")
+
 pytestmark = pytest.mark.gpu
 CURVES = ["bn254", "bls12381", "bls12377", "bls24315", "bls24317", "bw6633", "bw6761"]
 
 
 def _ev(p, x, r):
     return sum(c * pow(x, i, r) for i, c in enumerate(p)) % r
+
+
+@pytest.mark.parametrize("c", CURVES)
+def test_table_multiplicative_generator(c):
+    """the curve table's GeneratorFullMultiplicativeGroup is the one the library's Fr domain uses"""
+    d = import_module("gnark-crypto_b200.fft").NewDomain(c, 2)
+    cp = curves.CURVE_PARAMS[c]
+    try:
+        assert curves._fr_decode(d.FrMultiplicativeGen, cp.r) == [cp.mult_gen]
+    finally:
+        d.close()
 
 
 @pytest.mark.parametrize("c", CURVES)
@@ -89,7 +102,7 @@ def test_commit_lagrange(c):
     coeffs = np.ascontiguousarray(coeffs[idx])            # BitReverse on the host: natural-order coefficients
     digest = kzg.CommitLagrange(evals, pk, dom)
     assert np.array_equal(digest, kzg.Commit(coeffs, pk))
-    f_alpha = _ev(kzg._fr_decode(coeffs, r), alpha, r)
+    f_alpha = _ev(curves._fr_decode(coeffs, r), alpha, r)
     assert np.array_equal(digest, cref.scalar_mul(g, gen, f_alpha))
     pk.close()
     dom.close()

@@ -13,6 +13,8 @@ import pytest
 from oracle import cref
 from oracle import oracle as O
 
+curves = import_module("gnark-crypto_b200.curves")
+
 pytestmark = pytest.mark.gpu
 CURVES = ["bn254", "bls12381", "bls12377", "bls24315", "bls24317", "bw6633", "bw6761"]
 FIELD = {c: i for i, c in enumerate(CURVES)}      # GMSM_FR_*
@@ -68,14 +70,14 @@ def test_abi_divide_and_evaluate(c):
     cases.append([r - 1] * (t + 3))
     for coeffs in cases:
         n = len(coeffs)
-        f = kzg._fr_encode(coeffs, r)
+        f = curves._fr_encode(coeffs, r)
         d_f = _dev(f)
         for a in (0, 1, r - 1, rng.randrange(r)):
-            a_limbs = kzg._fr_encode([a], r)[0]
+            a_limbs = curves._fr_encode([a], r)[0]
             fa, h = _div(c, d_f, n, a_limbs)
             want = kzg._eval(coeffs, a, r)
-            assert np.array_equal(fa, kzg._fr_encode([want], r)[0]), (n, a)
-            assert np.array_equal(h, kzg._fr_encode(kzg._divide_by_x_minus_a(coeffs, want, a, r), r).reshape(-1, cp.fr_words)), (n, a)
+            assert np.array_equal(fa, curves._fr_encode([want], r)[0]), (n, a)
+            assert np.array_equal(h, curves._fr_encode(kzg._divide_by_x_minus_a(coeffs, want, a, r), r).reshape(-1, cp.fr_words)), (n, a)
             fa_only, _ = _div(c, d_f, n, a_limbs, quotient=False)
             assert np.array_equal(fa_only, fa), (n, a)
         assert np.array_equal(_host(d_f, cp.fr_words), f)
@@ -91,13 +93,13 @@ def test_abi_fold(c):
     for lens, gamma in (([3000, 17, 1, 1025], rng.randrange(r)), ([513], rng.randrange(r)), ([40, 900], 0),
                         ([33, 7, 1, 50, 2, 9, 64, 1, 12, 70, 5], r - 1)):
         polys = [[rng.randrange(r) for _ in range(m)] for m in lens]
-        d_polys = [_dev(kzg._fr_encode(p, r)) for p in polys]
+        d_polys = [_dev(curves._fr_encode(p, r)) for p in polys]
         out_len = max(lens)
         w = kzg.CURVE_PARAMS[c].fr_words
         d_out = torch.full((out_len * w,), -1, dtype=torch.int64, device="cuda")
         ptrs = (ctypes.c_void_p * len(polys))(*[d.data_ptr() for d in d_polys])
         ln = np.array(lens, dtype=np.uint64)
-        g = kzg._fr_encode([gamma], r)[0]
+        g = curves._fr_encode([gamma], r)[0]
         rc = _lib().gmsm_fr_poly_fold_device(FIELD[c], ptrs, ln.ctypes.data, len(polys), g.ctypes.data, d_out.data_ptr(), out_len,
                                              torch.cuda.current_stream().cuda_stream)
         assert rc == 0
@@ -106,7 +108,7 @@ def test_abi_fold(c):
             gi = pow(gamma, i, r)
             for j, v in enumerate(p):
                 want[j] = (want[j] + gi * v) % r
-        assert np.array_equal(_host(d_out, w), kzg._fr_encode(want, r)), (lens, gamma)
+        assert np.array_equal(_host(d_out, w), curves._fr_encode(want, r)), (lens, gamma)
 
 
 def test_abi_rejects_bad_arguments():
@@ -115,9 +117,9 @@ def test_abi_rejects_bad_arguments():
     L = _lib()
     nat = import_module("gnark-crypto_b200._native")
     r = kzg.CURVE_PARAMS["bn254"].r
-    d_f = _dev(kzg._fr_encode(list(range(1, 100)), r))
+    d_f = _dev(curves._fr_encode(list(range(1, 100)), r))
     d_fa = torch.empty(4, dtype=torch.int64, device="cuda")
-    a = kzg._fr_encode([7], r)[0]
+    a = curves._fr_encode([7], r)[0]
     assert L.gmsm_fr_poly_div_x_minus_a_device(0, d_f.data_ptr(), 0, a.ctypes.data, None, d_fa.data_ptr(), None, None) == nat.GMSM_EINVAL
     assert "n = 0" in nat.last_error()
     assert L.gmsm_fr_poly_div_x_minus_a_device(9, d_f.data_ptr(), 99, a.ctypes.data, None, d_fa.data_ptr(), None, None) == nat.GMSM_EINVAL
@@ -142,12 +144,12 @@ def test_large_closed_form(c, n):
     torch = _torch()
     cp = kzg.CURVE_PARAMS[c]
     r, w, t = cp.r, cp.fr_words, TILE[cp.fr_bytes]
-    one = torch.from_numpy(kzg._fr_encode([1], r)[0].view(np.int64).copy()).cuda()
+    one = torch.from_numpy(curves._fr_encode([1], r)[0].view(np.int64).copy()).cuda()
     d_f = one.repeat(n)
     a = 0x1234567890ABCDEF1234567 % r
-    fa, h = _div(c, d_f, n, kzg._fr_encode([a], r)[0])
+    fa, h = _div(c, d_f, n, curves._fr_encode([a], r)[0])
     inv = pow(a - 1, -1, r)
-    assert np.array_equal(fa, kzg._fr_encode([(pow(a, n, r) - 1) * inv % r], r)[0])
+    assert np.array_equal(fa, curves._fr_encode([(pow(a, n, r) - 1) * inv % r], r)[0])
     rng = random.Random(n)
     idx = {0, n - 2, 1, t - 2, t - 1, t, t * t - 1, t * t, t * t - 2}
     for k in range(1, 40):
@@ -155,9 +157,9 @@ def test_large_closed_form(c, n):
     while len(idx) < 256:
         idx.add(rng.randrange(n - 1))
     idx = sorted(idx)
-    want = kzg._fr_encode([(pow(a, n - 1 - i, r) - 1) * inv % r for i in idx], r)
+    want = curves._fr_encode([(pow(a, n - 1 - i, r) - 1) * inv % r for i in idx], r)
     assert np.array_equal(h[idx], want)
-    fa_only, _ = _div(c, d_f, n, kzg._fr_encode([a], r)[0], quotient=False)
+    fa_only, _ = _div(c, d_f, n, curves._fr_encode([a], r)[0], quotient=False)
     assert np.array_equal(fa_only, fa)
     assert bool((d_f.view(-1, w) == one).all())
 
@@ -189,7 +191,7 @@ def _check_open(c, pk, gen, alpha, coeffs, a):
     assert np.array_equal(op.H, cref.scalar_mul(g, gen, (_ev(coeffs, alpha, r) - fa) * pow(alpha - a, -1, r) % r))
     # the host path this replaces, on the same inputs
     h = kzg._divide_by_x_minus_a(coeffs, fa, a, r)
-    assert np.array_equal(op.H, kzg.Commit(kzg._fr_encode(h, r), pk))
+    assert np.array_equal(op.H, kzg.Commit(curves._fr_encode(h, r), pk))
     return op
 
 

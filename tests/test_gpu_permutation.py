@@ -12,6 +12,8 @@ import pytest
 from oracle import oracle as O
 from tests import permutation_ref as ref
 
+curves = import_module("gnark-crypto_b200.curves")
+
 pytestmark = pytest.mark.gpu
 CURVES = ["bn254", "bls12381", "bls12377", "bls24315", "bls24317", "bw6633", "bw6761"]
 FIELD = {c: i for i, c in enumerate(CURVES)}
@@ -39,7 +41,7 @@ def _host(t, w):
 
 def _enc(vals, c):
     kzg = _mods()[0]
-    return kzg._fr_encode(vals, kzg.CURVE_PARAMS[c].r)
+    return curves._fr_encode(vals, kzg.CURVE_PARAMS[c].r)
 
 
 def _stream():
@@ -214,7 +216,7 @@ def _assert_equal_ref(proof, want, c):
     kzg = _mods()[0]
     r = kzg.CURVE_PARAMS[c].r
     assert proof.size == want["size"]
-    assert kzg._fr_decode(proof.g, r)[0] == want["g"]
+    assert curves._fr_decode(proof.g, r)[0] == want["g"]
     for name in ("t1", "t2", "z", "q"):
         assert np.array_equal(proof.__dict__[name], want[name]), name
     assert np.array_equal(proof.batchedProof.H, want["H"])
@@ -238,7 +240,7 @@ def test_prove_equals_restatement(c):
     srs = ref.ClosedFormSRS(c, size, alpha)
     cases = [_reference_vectors(c)] + [_rand_perm(c, n, 100 * FIELD[c] + n) for n in (2, 4, 1 << 10)]
     for k, (a, b) in enumerate(cases):
-        want = ref.prove(c, kzg._fr_decode(a, r), kzg._fr_decode(b, r), srs)
+        want = ref.prove(c, curves._fr_decode(a, r), curves._fr_decode(b, r), srs)
         keep = (a.copy(), b.copy())
         _assert_equal_ref(perm.Prove(pk, a, b), want, c)
         assert np.array_equal(a, keep[0]) and np.array_equal(b, keep[1])
@@ -300,14 +302,21 @@ def test_device_path_taken(monkeypatch):
     alpha = 987654321
     pk, pkw = _pk(c, 256, alpha), _pk(c, 256, alpha, window_tables=True)
     a, b = _rand_perm(c, 256, 5)
-    want = ref.prove(c, kzg._fr_decode(a, r), kzg._fr_decode(b, r), ref.ClosedFormSRS(c, 256, alpha))
+    want = ref.prove(c, curves._fr_decode(a, r), curves._fr_decode(b, r), ref.ClosedFormSRS(c, 256, alpha))
 
     def boom(*args, **kw):
         raise AssertionError("host path called")
 
     for name in ("_eval", "_divide_by_x_minus_a"):
         monkeypatch.setattr(kzg, name, boom)
-    monkeypatch.setattr(perm, "_host", boom)
+    host_poly = kzg._host_poly
+
+    def host_arrays_only(p, words):     # a device polynomial brought back to the host is the sharded-key path
+        if kzg._is_device(p):
+            boom()
+        return host_poly(p, words)
+
+    monkeypatch.setattr(kzg, "_host_poly", host_arrays_only)
     monkeypatch.setattr(fft.Domain, "FFT", boom)
     monkeypatch.setattr(fft.Domain, "FFTInverse", boom)
     for key in (pk, pkw):
@@ -332,6 +341,6 @@ def test_sharded_key(monkeypatch):
     pk = _pk(c, 1 << 10, alpha, device=-1)
     for n in (8, 1 << 10):
         a, b = _rand_perm(c, n, 77 + n)
-        want = ref.prove(c, kzg._fr_decode(a, r), kzg._fr_decode(b, r), ref.ClosedFormSRS(c, 1 << 10, alpha))
+        want = ref.prove(c, curves._fr_decode(a, r), curves._fr_decode(b, r), ref.ClosedFormSRS(c, 1 << 10, alpha))
         _assert_equal_ref(perm.Prove(pk, a, b), want, c)
     pk.close()

@@ -15,6 +15,8 @@ from tests import shplonk_ref as ref
 from tests.test_emu_lincomb_cpu import cases as lincomb_cases
 from tests.test_emu_lincomb_cpu import lincomb_ref
 
+curves = import_module("gnark-crypto_b200.curves")
+
 pytestmark = pytest.mark.gpu
 CURVES = ["bn254", "bls12381", "bls12377", "bls24315", "bls24317", "bw6633", "bw6761"]
 FIELD = {c: i for i, c in enumerate(CURVES)}
@@ -42,7 +44,7 @@ def _lincomb(c, d_polys, lens, scalars, strides, offsets, d_out, out_len, accumu
     r = kzg.CURVE_PARAMS[c].r
     ptrs = (ctypes.c_void_p * len(d_polys))(*[d.data_ptr() if d is not None else None for d in d_polys])
     ln, st, off = (np.array(v, dtype=np.uint64) for v in (lens, strides, offsets))
-    sc = scalars if isinstance(scalars, np.ndarray) else kzg._fr_encode(scalars, r)
+    sc = scalars if isinstance(scalars, np.ndarray) else curves._fr_encode(scalars, r)
     return nat.lib().gmsm_fr_poly_lincomb_device(FIELD[c], ptrs, ln.ctypes.data, sc.ctypes.data, st.ctypes.data, off.ctypes.data,
                                                   len(d_polys), d_out.data_ptr() if d_out is not None else None, out_len,
                                                   accumulate, _torch().cuda.current_stream().cuda_stream)
@@ -59,13 +61,13 @@ def test_abi_lincomb(c):
     rng = random.Random(61 + FIELD[c])
     for lens, scalars, strides, offsets, out_len in lincomb_cases(r, rng) + [([70000, 3], [rng.randrange(r), 1], [3, 1], [2, 0], 210003)]:
         polys = [[rng.randrange(r) for _ in range(m)] for m in lens]
-        enc = [kzg._fr_encode(p, r) for p in polys]
+        enc = [curves._fr_encode(p, r) for p in polys]
         d_polys = [_dev(e) for e in enc]
         for init in (None, [rng.randrange(r) for _ in range(out_len)]):
-            d_out = _dev(kzg._fr_encode(init, r)) if init else torch.full((out_len * w,), -1, dtype=torch.int64, device="cuda")
+            d_out = _dev(curves._fr_encode(init, r)) if init else torch.full((out_len * w,), -1, dtype=torch.int64, device="cuda")
             assert _lincomb(c, d_polys, lens, scalars, strides, offsets, d_out, out_len, 1 if init else 0) == 0
             want = lincomb_ref(polys, scalars, strides, offsets, out_len, r, init)
-            assert np.array_equal(_host(d_out, w), kzg._fr_encode(want, r)), (lens, strides, offsets)
+            assert np.array_equal(_host(d_out, w), curves._fr_encode(want, r)), (lens, strides, offsets)
         assert all(np.array_equal(_host(d, w), e) for d, e in zip(d_polys, enc))
 
 
@@ -74,7 +76,7 @@ def test_abi_lincomb_rejects_bad_arguments():
     torch = _torch()
     nat = import_module("gnark-crypto_b200._native")
     r = kzg.CURVE_PARAMS["bn254"].r
-    d_f = _dev(kzg._fr_encode(list(range(1, 100)), r))
+    d_f = _dev(curves._fr_encode(list(range(1, 100)), r))
     d_out = torch.zeros(400, dtype=torch.int64, device="cuda")
     ok = dict(lens=[99], scalars=[3], strides=[1], offsets=[0])
 
@@ -101,7 +103,7 @@ def test_abi_lincomb_rejects_bad_arguments():
         ptrs = (ctypes.c_void_p * 1)(d_f.data_ptr())
         ln = np.array([99], dtype=np.uint64)
         one = np.array([1], dtype=np.uint64)
-        sc = kzg._fr_encode([3], r)
+        sc = curves._fr_encode([3], r)
         return nat.lib().gmsm_fr_poly_lincomb_device(f, ptrs, ln.ctypes.data, sc.ctypes.data, one.ctypes.data, one.ctypes.data, 1,
                                                       d_out.data_ptr(), 100, 0, None)
 
@@ -140,13 +142,13 @@ def _rand_limbs(n, c, seed):
 def _points_enc(c, sets):
     kzg = _mods()[0]
     r = kzg.CURVE_PARAMS[c].r
-    return [kzg._fr_encode(S, r).reshape(-1, kzg.CURVE_PARAMS[c].fr_words) for S in sets]
+    return [curves._fr_encode(S, r).reshape(-1, kzg.CURVE_PARAMS[c].fr_words) for S in sets]
 
 
 def _host_shplonk(c, pk, polys_limbs, sets, digests, hf, *data):
     kzg, shplonk, _ = _mods()
     r = kzg.CURVE_PARAMS[c].r
-    polys = [kzg._fr_decode(p, r) for p in polys_limbs]
+    polys = [curves._fr_decode(p, r) for p in polys_limbs]
     return shplonk.batch_open_host(polys, sets, digests, hf, c, shplonk._host_commit(pk), *data)
 
 
@@ -154,7 +156,7 @@ def _assert_proof(proof, want, c):
     kzg = _mods()[0]
     r = kzg.CURVE_PARAMS[c].r
     assert np.array_equal(proof.W, want[0]) and np.array_equal(proof.WPrime, want[1])
-    assert [kzg._fr_decode(v, r) if len(v) else [] for v in proof.ClaimedValues] == want[2]
+    assert [curves._fr_decode(v, r) if len(v) else [] for v in proof.ClaimedValues] == want[2]
 
 
 @pytest.mark.parametrize("c", CURVES)
@@ -183,19 +185,19 @@ def test_shplonk_fflonk_small_equal_host(c):
         ext = [fflonk._extend_set(S, t, c) for S, t in zip(sets, ts)]
         folded = [fflonk.Fold(p, c) for p in packs]
         _assert_proof(proof.SOpeningProof, _host_shplonk(c, pk, folded, ext, dig, hf, *data), c)
-        outer = [[kzg._fr_decode(v, r) for v in vals] for vals in proof.ClaimedValues]
-        assert ref.fflonk_fold_consistent(outer, [kzg._fr_decode(v, r) for v in proof.SOpeningProof.ClaimedValues], sets, c)
+        outer = [[curves._fr_decode(v, r) for v in vals] for vals in proof.ClaimedValues]
+        assert ref.fflonk_fold_consistent(outer, [curves._fr_decode(v, r) for v in proof.SOpeningProof.ClaimedValues], sets, c)
         for vals, pack, S, t in zip(outer, packs, sets, ts):
             assert len(vals) == t
             for i, p in enumerate(pack):
-                assert vals[i] == [shplonk._eval(kzg._fr_decode(p, r), pow(s, t, r), r) for s in S]
+                assert vals[i] == [shplonk._eval(curves._fr_decode(p, r), pow(s, t, r), r) for s in S]
     pk.close()
 
 
 def _verify(c, pk_alpha, polys, sets, proof, digests, hf, *data):
     kzg = _mods()[0]
     r = kzg.CURVE_PARAMS[c].r
-    claimed = [kzg._fr_decode(v, r) if len(v) else [] for v in proof.ClaimedValues]
+    claimed = [curves._fr_decode(v, r) if len(v) else [] for v in proof.ClaimedValues]
     return ref.verify_in_exponent(polys, sets, proof.W, proof.WPrime, claimed, digests, hf, c, pk_alpha, *data)
 
 
@@ -218,7 +220,7 @@ def test_verify_in_exponent(c, logn):
     proof = shplonk.BatchOpen(polys, digests, _points_enc(c, sets), hashlib.sha256, pk, b"plonk")
     assert _verify(c, alpha, None, sets, proof, digests, hashlib.sha256, b"plonk")
     proof.ClaimedValues[2] = proof.ClaimedValues[2].copy()
-    proof.ClaimedValues[2][1] = kzg._fr_encode([(kzg._fr_decode(proof.ClaimedValues[2][1:2], r)[0] + 1) % r], r)[0]
+    proof.ClaimedValues[2][1] = curves._fr_encode([(curves._fr_decode(proof.ClaimedValues[2][1:2], r)[0] + 1) % r], r)[0]
     assert not _verify(c, alpha, None, sets, proof, digests, hashlib.sha256, b"plonk")
     m = n // 4
     w = kzg.CURVE_PARAMS[c].fr_words
@@ -229,8 +231,8 @@ def test_verify_in_exponent(c, logn):
     ts = [fflonk._next_divisor_r_minus_one(len(p), r) for p in packs]
     ext = [fflonk._extend_set(S, t, c) for S, t in zip(fsets, ts)]
     assert _verify(c, alpha, None, ext, fp.SOpeningProof, dig, hashlib.blake2b)
-    outer = [[kzg._fr_decode(v, r) for v in vals] for vals in fp.ClaimedValues]
-    assert ref.fflonk_fold_consistent(outer, [kzg._fr_decode(v, r) for v in fp.SOpeningProof.ClaimedValues], fsets, c)
+    outer = [[curves._fr_decode(v, r) for v in vals] for vals in fp.ClaimedValues]
+    assert ref.fflonk_fold_consistent(outer, [curves._fr_decode(v, r) for v in fp.SOpeningProof.ClaimedValues], fsets, c)
     assert all(torch.equal(a, b) for a, b in zip(polys, keep))
     pk.close()
 

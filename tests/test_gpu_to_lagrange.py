@@ -14,6 +14,8 @@ import pytest
 
 from tests import lagrange_ref as LR
 
+curves = import_module("gnark-crypto_b200.curves")
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIBDIR = os.path.join(ROOT, "gnark-crypto_b200")
@@ -143,7 +145,7 @@ def test_commit_with_lagrange_key(curve):
     r = LR.fr_modulus(curve)
     rng = random.Random(99)
     P = _bsm(curve, _gen(curve), [rng.randrange(1, r) for _ in range(n)])
-    evals = kzg._fr_encode([rng.randrange(r) for _ in range(n)], r)
+    evals = curves._fr_encode([rng.randrange(r) for _ in range(n)], r)
     pk_lag = kzg.ProvingKey(curve, kzg.ToLagrangeG1(P, curve))
     pk = kzg.ProvingKey(curve, P)
     dom = fft.NewDomain(curve, n)
@@ -171,7 +173,7 @@ def test_errors():
     for cname in ("bn254_g2", "bls12381_g2", "bls12377_g2", "bw6761_g2", "bw6633_g2", "secp256k1_g1"):
         cid = mx.CURVES[cname]
         assert L.gmsm_g1_to_lagrange_workspace_bytes(cid, 4) == 0
-        pts = np.zeros((4, 2 * mx._words(cid)), dtype=np.uint64)
+        pts = np.zeros((4, 2 * curves.GROUPS[cname].words), dtype=np.uint64)
         with pytest.raises(mx.MultiExpError, match="pairing curves only"):
             kzg.ToLagrangeG1(pts, cname)
 

@@ -6,6 +6,8 @@ import struct
 import numpy as np
 import pytest
 
+curves = importlib.import_module("gnark-crypto_b200.curves")
+
 
 def test_slice_roundtrip_and_limits():
     kzg = importlib.import_module("gnark-crypto_b200.kzg")
@@ -39,7 +41,8 @@ def test_open_host_polynomial_arithmetic():
 
     kzg = importlib.import_module("gnark-crypto_b200.kzg")
     rng = random.Random(7)
-    for name, r in kzg.FR_MODULUS.items():
+    for cp in kzg.CURVE_PARAMS.values():
+        r = cp.r
         f = [rng.randrange(r) for _ in range(37)]
         a = rng.randrange(r)
         fa = kzg._eval(f, a, r)
@@ -48,10 +51,10 @@ def test_open_host_polynomial_arithmetic():
         assert len(h) == len(f) - 1
         for x in (0, 1, rng.randrange(r)):
             assert (kzg._eval(h, x, r) * (x - a) + fa) % r == kzg._eval(f, x, r)
-        enc = kzg._fr_encode(f, r)
-        assert kzg._fr_decode(enc, r) == f
+        enc = curves._fr_encode(f, r)
+        assert curves._fr_decode(enc, r) == f
     # fr.One of bn254 in Montgomery form (ecc/bn254/fr/element.go:227)
-    one = kzg._fr_encode([1], kzg.FR_MODULUS["bn254"])[0]
+    one = curves._fr_encode([1], kzg.CURVE_PARAMS["bn254"].r)[0]
     assert [int(x) for x in one] == [12436184717236109307, 3962172157175319849, 7381016538464732718, 1011752739694698287]
 
 
@@ -74,15 +77,15 @@ def test_point_marshal_host_restatement():
         for m in range(1, 40):
             P = G.encode_affine([G.scalar_mul(G.gen, m * 7919)])[0]
             cb, rb = kzg.g1_bytes(P, c), kzg.g1_raw_bytes(P, c)
-            seen.add(cb[0] & kzg._FLAGS[c]["mask"])
+            seen.add(cb[0] & kzg.CURVE_PARAMS[c].flags["mask"])
             for b in (cb, rb):
                 q, used = kzg.g1_set_bytes(b + b"trailing", c)
                 assert np.array_equal(q, P) and used == len(b)
             x, y = G.decode_affine(P.reshape(1, -1))[0]
             assert int.from_bytes(rb[: len(rb) // 2], "big") == int(x) and int.from_bytes(rb[len(rb) // 2 :], "big") == int(y)
-        assert seen == {kzg._FLAGS[c]["small"], kzg._FLAGS[c]["large"]}
+        assert seen == {kzg.CURVE_PARAMS[c].flags["small"], kzg.CURVE_PARAMS[c].flags["large"]}
         z = np.zeros_like(P)
-        assert kzg.g1_bytes(z, c)[0] == kzg._FLAGS[c]["inf"] and not any(kzg.g1_bytes(z, c)[1:])
+        assert kzg.g1_bytes(z, c)[0] == kzg.CURVE_PARAMS[c].flags["inf"] and not any(kzg.g1_bytes(z, c)[1:])
         for b in (kzg.g1_bytes(z, c), kzg.g1_raw_bytes(z, c)):
             q, used = kzg.g1_set_bytes(b, c)
             assert not q.any() and used == len(b)
@@ -91,7 +94,7 @@ def test_point_marshal_host_restatement():
         with pytest.raises(ValueError, match="invalid infinity point encoding"):
             kzg.g1_set_bytes(bytes(bad), c)
         with pytest.raises(ValueError, match="invalid fp.Element encoding"):
-            kzg.g1_set_bytes(bytes([kzg._FLAGS[c]["small"] | (~kzg._FLAGS[c]["mask"] & 0xFF)] + [0xFF] * (len(bad) - 1)), c)
+            kzg.g1_set_bytes(bytes([kzg.CURVE_PARAMS[c].flags["small"] | (~kzg.CURVE_PARAMS[c].flags["mask"] & 0xFF)] + [0xFF] * (len(bad) - 1)), c)
 
 
 def test_derive_gamma_transcript():

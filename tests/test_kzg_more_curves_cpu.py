@@ -10,6 +10,8 @@ import pytest
 
 from oracle import oracle as O
 
+curves = importlib.import_module("gnark-crypto_b200.curves")
+
 ALL = ["bn254", "bls12381", "bls12377", "bls24315", "bls24317", "bw6633", "bw6761"]
 NEW = ["bls24315", "bls24317", "bw6633", "bw6761"]
 # (fr.Limbs, fp.Limbs, q mod 4) as the reference states them (fr|fp/element.go:41)
@@ -24,24 +26,36 @@ def _kzg():
 @pytest.mark.parametrize("c", ALL)
 def test_curve_table(c):
     kzg = _kzg()
-    me = importlib.import_module("gnark-crypto_b200.multiexp")
     cp = kzg.CURVE_PARAMS[c]
     G = O.GROUPS[c + "_g1"]
     fr_words, fp_words, qmod4 = SIZES[c]
     assert (cp.fr_words, cp.fp_words, cp.q % 4) == (fr_words, fp_words, qmod4)
     assert (cp.fr_bytes, cp.fp_bytes) == (8 * fr_words, 8 * fp_words)
     assert cp.r == G.fr.q and cp.q == G.K.q and cp.b == G.b % cp.q
-    assert kzg._limbs(cp.r) == cp.fr_words and kzg._limbs(cp.q) == cp.fp_words
-    cid = me.CURVES[c + "_g1"]
-    assert me.SCALAR_WORDS[cid] == cp.fr_words and me._words(cid) == cp.fp_words
+    assert curves._limbs(cp.r) == cp.fr_words and curves._limbs(cp.q) == cp.fp_words
+    g1 = curves.GROUPS[c + "_g1"]
+    assert g1.scalar_words == cp.fr_words and g1.words == cp.fp_words
     x, y = G.gen
     assert (x ** 3 + cp.b - y * y) % cp.q == 0                   # the generator is on y^2 = x^3 + b
     assert cp.flags["mask"] == (0b11 << 6 if c == "bn254" else 0b111 << 5)
-    assert kzg.FR_MODULUS[c] == cp.r and kzg.FP_MODULUS[c] == cp.q and kzg.CURVE_B[c] == cp.b and kzg._FLAGS[c] is cp.flags
     # the scalar codec sizes itself from r
     vals = [0, 1, cp.r - 1, 123456789]
-    enc = kzg._fr_encode(vals, cp.r)
-    assert enc.shape == (4, cp.fr_words) and np.array_equal(enc, G.encode_scalars(vals)) and kzg._fr_decode(enc, cp.r) == vals
+    enc = curves._fr_encode(vals, cp.r)
+    assert enc.shape == (4, cp.fr_words) and np.array_equal(enc, G.encode_scalars(vals)) and curves._fr_decode(enc, cp.r) == vals
+
+
+def test_group_table_matches_library_and_oracle():
+    """the one curve table against the library's layout queries and the oracle (pure host calls): every group's affine point and
+    scalar sizes and its scalar bits, every pairing curve's GMSM_FR_* element size"""
+    L = importlib.import_module("gnark-crypto_b200._native").lib()
+    assert sorted(g.id for g in curves.GROUPS.values()) == list(range(13))
+    for name, g in curves.GROUPS.items():
+        assert L.gmsm_affine_bytes(g.id) == 16 * g.words, name
+        assert L.gmsm_scalar_bytes(g.id) == 8 * g.scalar_words, name
+        assert g.scalar_bits == O.GROUPS[name].fr.bits, name
+    assert sorted(cp.fr_id for cp in curves.CURVE_PARAMS.values()) == list(range(7))
+    for c, cp in curves.CURVE_PARAMS.items():
+        assert L.gmsm_fft_fr_bytes(cp.fr_id) == cp.fr_bytes, c
 
 
 def test_bw6761_b_is_minus_one():

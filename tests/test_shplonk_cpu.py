@@ -11,6 +11,8 @@ import pytest
 
 from tests import shplonk_ref as ref
 
+curves = import_module("gnark-crypto_b200.curves")
+
 CURVES = ["bn254", "bls12381", "bls12377", "bls24315", "bls24317", "bw6633", "bw6761"]
 
 
@@ -68,7 +70,7 @@ def test_fflonk_identities_equal_reference(c):
         ts = [fflonk._next_divisor_r_minus_one(len(pk), r) for pk in packs]
         assert all(t >= len(pk) and (r - 1) % t == 0 for t, pk in zip(ts, packs))
         ext = [fflonk._extend_set(S, t, c) for S, t in zip(pts, ts)]
-        folded = [kzg._fr_decode(fflonk.Fold([kzg._fr_encode(p, r) for p in pk], c), r) for pk in packs]
+        folded = [curves._fr_decode(fflonk.Fold([curves._fr_encode(p, r) for p in pk], c), r) for pk in packs]
         digests = _digests(srs, folded)
         want = shplonk.batch_open_host(folded, ext, digests, hashlib.sha256, c, srs.commit)
         got = ref.identity_open(packs, pts, ts, ext, digests, hashlib.sha256, c, srs.commit)
@@ -84,7 +86,7 @@ def test_fflonk_identities_equal_reference(c):
         pk3 = [[rng.randrange(r) for _ in range(4)] for _ in range(3)]
         S = [s[0], s[0] * omega % r]
         ext = [fflonk._extend_set(S, 3, c)]
-        folded = [kzg._fr_decode(fflonk.Fold([kzg._fr_encode(p, r) for p in pk3], c), r)]
+        folded = [curves._fr_decode(fflonk.Fold([curves._fr_encode(p, r) for p in pk3], c), r)]
         digests = _digests(srs, folded)
         want = shplonk.batch_open_host(folded, ext, digests, hashlib.sha256, c, srs.commit)
         got = ref.identity_open([pk3], [S], [3], ext, digests, hashlib.sha256, c, srs.commit)

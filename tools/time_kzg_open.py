@@ -37,6 +37,7 @@ def main():
     import gnark_crypto_b200  # noqa: F401
 
     kzg = importlib.import_module("gnark-crypto_b200.kzg")
+    curves = importlib.import_module("gnark-crypto_b200.curves")
     mx = importlib.import_module("gnark-crypto_b200.multiexp")
     gens = json.load(open(os.path.join(ROOT, "gnark-crypto_b200", "generators.json")))
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
@@ -81,12 +82,12 @@ def main():
         p[:, w - 1] = 0                                     # < r: arbitrary Montgomery residues
         a = p[12345].copy()
         d_p = kzg._device_poly(p, w, 0)
-        dp = kzg._DevicePoly(pk, n)
+        dp = kzg._DevicePoly(curve, 0, n)
         d_h, d_fa = dp.empty(n - 1), dp.empty(1)
         d_fold = dp.empty(n)
         d_claimed = dp.empty(args.k)
         polys_t = [d_p] * args.k
-        gamma = kzg._reduced(p[777], cp.r)
+        gamma = curves._reduced(p[777], cp.r)
         res = {"curve": curve, "logn": logn, "fr_bytes": S, "k": args.k, "reps": args.reps}
         res["upload_ms"] = timed(lambda: kzg._device_poly(p, w, 0))
         res["scan_ms"] = timed(lambda: dp.div(d_p, n, a, d_h, d_fa))
@@ -105,11 +106,11 @@ def main():
         res["batch_open_tensor_ms"] = wall(lambda: kzg.BatchOpenSinglePoint(polys_t, digests, a, hashlib.sha256, pk))
         if args.host_ref and logn == 20:
             t0 = time.perf_counter()
-            coeffs = kzg._fr_decode(p, cp.r)
-            av = kzg._fr_decode(a, cp.r)[0]
+            coeffs = curves._fr_decode(p, cp.r)
+            av = curves._fr_decode(a, cp.r)[0]
             fa = kzg._eval(coeffs, av, cp.r)
             h = kzg._divide_by_x_minus_a(coeffs, fa, av, cp.r)
-            kzg._fr_encode(h, cp.r)
+            curves._fr_encode(h, cp.r)
             res["host_fr_loops_ms"] = (time.perf_counter() - t0) * 1e3
         print(json.dumps({k: (round(v, 4) if isinstance(v, float) else v) for k, v in res.items()}), flush=True)
         pk.close()

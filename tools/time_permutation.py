@@ -68,7 +68,7 @@ def main():
     kzg = import_module("gnark-crypto_b200.kzg")
     perm = import_module("gnark-crypto_b200.permutation")
     fft = import_module("gnark-crypto_b200.fft")
-    nat = import_module("gnark-crypto_b200._native")
+    curves = import_module("gnark-crypto_b200.curves")
     from oracle import oracle as O
 
     print("card:", _card(), flush=True)
@@ -76,7 +76,6 @@ def main():
     for c in a.curves.split(","):
         cp = kzg.CURVE_PARAMS[c]
         r, w, fb = cp.r, cp.fr_words, cp.fr_bytes
-        field = fft._FIELDS[c]
         G = O.GROUPS[c + "_g1"]
         gen = G.encode_affine([G.gen])[0]
         pk = kzg.ProvingKey(c, kzg.new_srs_g1(c, 1 << max(logs), 0xC0FFEE % r, gen, r, G.encode_scalars))
@@ -112,19 +111,15 @@ def main():
                 for v in bufs[:2]:
                     pk._bases.MultiExpDevice(v, n - 1, stream=st)
 
-            L = nat.lib()
-            eps, om = kzg._fr_encode([0x1234567 % r], r)[0], kzg._fr_encode([0x7654321 % r], r)[0]
-            ws = int(L.gmsm_fr_permutation_workspace_bytes(field, n))
-            work = torch.empty(max(ws // 8, 1), dtype=torch.int64, device="cuda")
+            eps, om = curves._fr_encode([0x1234567 % r], r)[0], curves._fr_encode([0x7654321 % r], r)[0]
+            dp = kzg._DevicePoly(c, 0, n)
             d_z, d_out = torch.empty_like(t1), torch.empty_like(t1)
 
             def accumulate():
-                kzg._check(L.gmsm_fr_permutation_accumulate_device(field, t1.data_ptr(), t2.data_ptr(), n, eps.ctypes.data, d_z.data_ptr(),
-                                                                   work.data_ptr(), st))
+                dp.permutation_accumulate(t1, t2, n, eps, d_z)
 
             def numerator():
-                kzg._check(L.gmsm_fft_permutation_numerator_device(dom._h, bufs[0].data_ptr(), bufs[1].data_ptr(), bufs[2].data_ptr(), n,
-                                                                   eps.ctypes.data, om.ctypes.data, d_out.data_ptr(), st))
+                dp.permutation_numerator(dom, bufs[0], bufs[1], bufs[2], eps, om, d_out)
 
             fft_ms = _events_ms(ffts, a.repeat, torch)
             msm_ms = _events_ms(msms, a.repeat, torch)
@@ -139,7 +134,7 @@ def main():
                 "numerator_TBps": round(num_b / num_ms / 1e9, 3), "numerator_share_of_3.35TBps": round(num_b / num_ms / 1e9 / (HBM_BYTES_PER_S / 1e12), 3),
             }), flush=True)
             dom.close()
-            del t1, t2, bufs, d_z, d_out, work
+            del t1, t2, bufs, d_z, d_out, dp
             torch.cuda.empty_cache()
         pk.close()
 

@@ -49,6 +49,7 @@ def main():
     import torch
 
     kzg = import_module("gnark-crypto_b200.kzg")
+    curves = import_module("gnark-crypto_b200.curves")
     shplonk = import_module("gnark-crypto_b200.shplonk")
     fflonk = import_module("gnark-crypto_b200.fflonk")
     from oracle import oracle as O
@@ -72,7 +73,7 @@ def main():
 
     zeta = 0x1234567 % r
     omega = fflonk._ith_root_one(2, c)
-    enc = lambda S: kzg._fr_encode(S, r).reshape(-1, w)          # noqa: E731
+    enc = lambda S: curves._fr_encode(S, r).reshape(-1, w)          # noqa: E731
     st = torch.cuda.current_stream().cuda_stream
 
     polys = [rand(ns) for _ in range(8)]
