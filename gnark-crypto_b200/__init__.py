@@ -8,7 +8,7 @@ Layout:
                G1Affine/G1Jac/G2Affine/G2Jac .MultiExp(points, scalars, MultiExpConfig)
                (ecc/bn254/multiexp.go:20,32,345,357; ecc/ecc.go:107-110) + the device-level Engine
   dist.py      multi-GPU: one process per GPU, shard points/scalars, all-gather the per-window partials
-  fft.py, kzg.py, shplonk.py, fflonk.py, permutation.py, transcript.py: the Fr FFT and the KZG provers; kzg._DevicePoly is
+  fft.py, kzg.py, shplonk.py, fflonk.py, permutation.py, plookup.py, transcript.py: the Fr FFT and the KZG provers; kzg._DevicePoly is
                the one caller of the library's device Fr polynomial entry points
 """
 from . import _native  # noqa: F401

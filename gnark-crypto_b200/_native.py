@@ -71,6 +71,10 @@ _SIGNATURES = [
     ("gmsm_fr_permutation_workspace_bytes", sz, [i32, sz]),
     ("gmsm_fr_permutation_accumulate_device", i32, [i32, vp, vp, sz, vp, vp, vp, vp]),
     ("gmsm_fft_permutation_numerator_device", i32, [vp, vp, vp, vp, sz, vp, vp, vp, vp]),
+    ("gmsm_fr_sort_workspace_bytes", sz, [i32, sz]),
+    ("gmsm_fr_sort_device", i32, [i32, vp, sz, vp, vp, vp]),
+    ("gmsm_fr_plookup_accumulate_device", i32, [i32, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]),
+    ("gmsm_fft_plookup_numerator_device", i32, [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]),
     ("gmsm_g1_to_lagrange_workspace_bytes", sz, [i32, sz]),
     ("gmsm_g1_to_lagrange", i32, [i32, vp, sz, i32, vp]),
     ("gmsm_g1_to_lagrange_device", i32, [i32, vp, sz, vp, vp, vp]),

@@ -23,6 +23,10 @@
 //   fr.BatchInvert                                ecc/bn254/fr/element.go:658-687
 //   evaluateAccumulationPolynomialBitReversed     ecc/bn254/fr/permutation/permutation.go:52-75
 //   the quotient numerator and its omega-fold     ecc/bn254/fr/permutation/permutation.go:78-121, 206-214
+// and the Fr steps of plookup.ProveLookupVector (kernels and the sort's schedule in plookup_kernels.cuh):
+//   sort.Sort(fr.Vector)                          ecc/bn254/fr/element.go:254 (fr.Element.Cmp)
+//   evaluateAccumulationPolynomial                ecc/bn254/fr/plookup/vector.go:52-95
+//   the quotient numerator and its alpha-fold     ecc/bn254/fr/plookup/vector.go:97-335
 #include <cuda_runtime.h>
 
 #include <cstdio>
@@ -38,6 +42,7 @@ using namespace gmsm;
 #include "fft_kernels.cuh"
 #include "poly_kernels.cuh"
 #include "perm_kernels.cuh"
+#include "plookup_kernels.cuh"
 
 namespace {
 
@@ -514,6 +519,128 @@ extern "C" int gmsm_fft_permutation_numerator_device(gmsm_fft_domain_t* d, const
     k_perm_numerator<P><<<perm_inv_tiles(n), PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), (cudaStream_t)stream>>>(
         reinterpret_cast<const F*>(d_lt1), reinterpret_cast<const F*>(d_lt2), reinterpret_cast<const F*>(d_lz), n, d->logn, k,
         reinterpret_cast<const F*>(d->d_tw), PERM_INV_LOG_T, reinterpret_cast<F*>(d_out));
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+// ---- sort.Sort(fr.Vector) and the Fr steps of plookup.ProveLookupVector (vector.go:52-335) on device vectors ----
+
+extern "C" size_t gmsm_fr_sort_workspace_bytes(int fr_field, size_t n) {
+  if (!gmsm_fft_fr_bytes(fr_field) || n == 0) return 0;
+  size_t bytes = 0;
+  with_fr(fr_field, [&](auto tag) {
+    using P = typename decltype(tag)::type;
+    bytes = sort_layout<P>(n, SORT_LOG_R, SORT_LOG_B).bytes;
+    return GMSM_OK;
+  });
+  return bytes;
+}
+
+extern "C" int gmsm_fr_sort_device(int fr_field, const void* d_in, size_t n, void* d_out, void* d_work, void* stream) {
+  const size_t fb = gmsm_fft_fr_bytes(fr_field);
+  if (!fb) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0) return set_err(GMSM_EINVAL, "empty vector (n = 0)");
+  if (!d_in || !d_out) return set_err(GMSM_EINVAL, "null vector");
+  if (!d_work) return set_err(GMSM_EINVAL, "null workspace (gmsm_fr_sort_workspace_bytes)");
+  if (n >= 0x80000000ull) return set_err(GMSM_EINVAL, "vector too large (n = %zu)", n);
+  if (d_out != d_in && overlaps(d_in, n * fb, d_out, n * fb)) return set_err(GMSM_EINVAL, "the output must equal the input or not overlap it");
+  const size_t wb = gmsm_fr_sort_workspace_bytes(fr_field, n);
+  if (overlaps(d_work, wb, d_in, n * fb) || overlaps(d_work, wb, d_out, n * fb))
+    return set_err(GMSM_EINVAL, "the workspace must not overlap the input or the output");
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    cudaStream_t st = (cudaStream_t)stream;
+    int err = GMSM_OK;
+    fr_sort_schedule<P>(
+        reinterpret_cast<const F*>(d_in), n, reinterpret_cast<F*>(d_out), reinterpret_cast<unsigned char*>(d_work), SORT_LOG_R, SORT_LOG_B,
+        [&](auto kernel, unsigned grid, unsigned block, auto... args) { kernel<<<grid, block, 0, st>>>(args...); },
+        [&](uint32_t* host, const uint32_t* dev, int words) {   // which byte positions vary decides the passes: one small copy
+          if (err == GMSM_OK && (cudaMemcpyAsync(host, dev, words * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+                                 cudaStreamSynchronize(st) != cudaSuccess))
+            err = set_err(GMSM_ECUDA, "reading the sort's difference mask: %s", cudaGetErrorString(cudaGetLastError()));
+          if (err != GMSM_OK) memset(host, 0, words * 4);
+        });
+    if (err != GMSM_OK) return err;
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fr_plookup_accumulate_device(int fr_field, const void* d_f, const void* d_t, const void* d_h1, const void* d_h2,
+                                                 size_t n, const uint64_t* beta, const uint64_t* gamma, void* d_z, void* d_work,
+                                                 void* stream) {
+  const size_t fb = gmsm_fft_fr_bytes(fr_field);
+  if (!fb) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0) return set_err(GMSM_EINVAL, "empty vector (n = 0)");
+  if (!d_f || !d_t || !d_h1 || !d_h2 || !d_z || !beta || !gamma) return set_err(GMSM_EINVAL, "null vector or challenge");
+  const size_t bytes = n * fb;
+  for (const void* in : {d_f, d_t, d_h1, d_h2})
+    if (overlaps(d_z, bytes, in, bytes)) return set_err(GMSM_EINVAL, "z must not overlap f, t, h1 or h2");
+  if (!d_work && gmsm_fr_permutation_workspace_bytes(fr_field, n))
+    return set_err(GMSM_EINVAL, "null workspace (gmsm_fr_permutation_workspace_bytes)");
+  if (((n - 1) >> PERM_INV_LOG_T) >= 0x7fffffffull) return set_err(GMSM_EINVAL, "vector too large (n = %zu)", n);
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    PlookupConsts<P> k;
+    if (!read_reduced(beta, &k.beta)) return set_err(GMSM_EINVAL, "beta is not a reduced fr.Element");
+    if (!read_reduced(gamma, &k.gamma)) return set_err(GMSM_EINVAL, "gamma is not a reduced fr.Element");
+    k.opb = fp_add(F::one(), k.beta);
+    k.gopb = fp_mul(k.gamma, k.opb);
+    cudaStream_t st = (cudaStream_t)stream;
+    F* z = reinterpret_cast<F*>(d_z);
+    k_plookup_ratio<P><<<perm_inv_tiles(n), PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), st>>>(
+        reinterpret_cast<const F*>(d_f), reinterpret_cast<const F*>(d_t), reinterpret_cast<const F*>(d_h1), reinterpret_cast<const F*>(d_h2),
+        n, k, PERM_INV_LOG_T, z);
+    constexpr int log_l = poly_log_l<P>(), log_b = poly_log_b<P>();
+    const size_t smem = poly_smem_bytes<P>(log_l, log_b);
+    perm_prefix_schedule<P>(
+        z, n, reinterpret_cast<F*>(d_work), log_l, log_b,
+        [&](const F* x, uint64_t m, F* heads, uint64_t tiles) {
+          k_perm_prod_heads<P><<<(unsigned)tiles, 1u << log_b, smem, st>>>(x, m, log_l, heads);
+        },
+        [&](F* x, uint64_t m, const F* carry, uint64_t tiles) {
+          k_perm_prod_write<P><<<(unsigned)tiles, 1u << log_b, smem, st>>>(x, m, log_l, carry);
+        });
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fft_plookup_numerator_device(gmsm_fft_domain_t* d, const void* d_lz, const void* d_lh1, const void* d_lh2,
+                                                 const void* d_lt, const void* d_lf, size_t n, const uint64_t* beta, const uint64_t* gamma,
+                                                 const uint64_t* alpha, void* d_out, void* stream) {
+  if (!d) return set_err(GMSM_EINVAL, "null domain");
+  if (n != d->n) return set_err(GMSM_EINVAL, "len(a) = %zu must equal the domain cardinality %llu", n, (unsigned long long)d->n);
+  if (!d_lz || !d_lh1 || !d_lh2 || !d_lt || !d_lf || !d_out || !beta || !gamma || !alpha)
+    return set_err(GMSM_EINVAL, "null vector or challenge");
+  const size_t bytes = n * 8 * (size_t)d->words;
+  for (const void* in : {d_lz, d_lh1, d_lh2, d_lt, d_lf})
+    if (overlaps(d_out, bytes, in, bytes)) return set_err(GMSM_EINVAL, "the output must not overlap lz, lh1, lh2, lt or lf");
+  std::lock_guard<std::mutex> lk(d->mu);
+  CK(cudaSetDevice(d->device));
+  return with_fr(d->field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    PlookupNumConsts<P> k;
+    if (!read_reduced(beta, &k.c.beta)) return set_err(GMSM_EINVAL, "beta is not a reduced fr.Element");
+    if (!read_reduced(gamma, &k.c.gamma)) return set_err(GMSM_EINVAL, "gamma is not a reduced fr.Element");
+    if (!read_reduced(alpha, &k.alpha)) return set_err(GMSM_EINVAL, "alpha is not a reduced fr.Element");
+    k.c.opb = fp_add(F::one(), k.c.beta);
+    k.c.gopb = fp_mul(k.c.gamma, k.c.opb);
+    memcpy(k.shift.l, d->consts[3], sizeof(F));
+    // gg = (w^2)^(s-1) = w^(n-2) = w^-2 (vector.go:124-126); x^s on the coset is shift^s (-1)^i (vector.go:165-181)
+    F winv;
+    memcpy(winv.l, d->consts[1], sizeof(F));
+    k.gg = fp_sqr(winv);
+    const F ss = d->logn ? host_pow2k(k.shift, d->logn - 1) : k.shift;   // shift^(n/2)
+    k.xs_inv[0] = fp_inv(fp_sub(ss, F::one()));
+    k.xs_inv[1] = fp_inv(fp_neg(fp_add(ss, F::one())));
+    k_plookup_numerator<P><<<perm_inv_tiles(n), PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), (cudaStream_t)stream>>>(
+        reinterpret_cast<const F*>(d_lz), reinterpret_cast<const F*>(d_lh1), reinterpret_cast<const F*>(d_lh2), reinterpret_cast<const F*>(d_lt),
+        reinterpret_cast<const F*>(d_lf), n, d->logn, k, reinterpret_cast<const F*>(d->d_tw), PERM_INV_LOG_T, reinterpret_cast<F*>(d_out));
     CK(cudaGetLastError());
     return GMSM_OK;
   });

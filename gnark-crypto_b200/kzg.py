@@ -229,6 +229,25 @@ class _DevicePoly:
                                                                    domain.Cardinality, eps.ctypes.data, omega.ctypes.data,
                                                                    d_out.data_ptr(), self.stream))
 
+    def sort(self, d_in, n: int, d_out):
+        """d_out = d_in sorted ascending by canonical value (sort.Sort(fr.Vector)); d_out may be d_in.  Returns once the sort has
+        read back which byte positions vary."""
+        ws = int(_native.lib().gmsm_fr_sort_workspace_bytes(self.field, n))
+        work = self.torch.empty((ws + 7) // 8, dtype=self.torch.int64, device=self.dev)
+        _check(_native.lib().gmsm_fr_sort_device(self.field, d_in.data_ptr(), n, d_out.data_ptr(), work.data_ptr(), self.stream))
+
+    def plookup_accumulate(self, d_f, d_t, d_h1, d_h2, n: int, beta: np.ndarray, gamma: np.ndarray, d_z):
+        """d_z = the accumulation polynomial z of plookup.ProveLookupVector in natural order (n <= max_len)"""
+        _check(_native.lib().gmsm_fr_plookup_accumulate_device(
+            self.field, d_f.data_ptr(), d_t.data_ptr(), d_h1.data_ptr(), d_h2.data_ptr(), n, beta.ctypes.data, gamma.ctypes.data,
+            d_z.data_ptr(), None if self.work is None else self.work.data_ptr(), self.stream))
+
+    def plookup_numerator(self, domain, d_lz, d_lh1, d_lh2, d_lt, d_lf, beta: np.ndarray, gamma: np.ndarray, alpha: np.ndarray, d_out):
+        """d_out = the quotient of plookup.ProveLookupVector before its inverse FFT, on the coset of `domain` (the big domain)"""
+        _check(_native.lib().gmsm_fft_plookup_numerator_device(
+            domain._h, d_lz.data_ptr(), d_lh1.data_ptr(), d_lh2.data_ptr(), d_lt.data_ptr(), d_lf.data_ptr(), domain.Cardinality,
+            beta.ctypes.data, gamma.ctypes.data, alpha.ctypes.data, d_out.data_ptr(), self.stream))
+
 
 @dataclass
 class OpeningProof:

@@ -273,6 +273,31 @@ int gmsm_fr_permutation_accumulate_device(int fr_field, const void* d_t1, const 
 int gmsm_fft_permutation_numerator_device(gmsm_fft_domain_t* domain, const void* d_lt1, const void* d_lt2, const void* d_lz, size_t n,
                                           const uint64_t* epsilon, const uint64_t* omega, void* d_out, void* stream);
 
+/* ---- sort.Sort(fr.Vector) and the Fr steps of plookup.ProveLookupVector (ecc/bn254/fr/plookup/vector.go; the same for the
+ * other six scalar fields), with the conventions of the block above ---- */
+/* bytes of device workspace gmsm_fr_sort_device needs for n elements (0 for n = 0 or an unknown field) */
+size_t gmsm_fr_sort_workspace_bytes(int fr_field, size_t n);
+/* d_out = d_in sorted ascending by canonical value (fr.Element.Cmp, fr/element.go:254), in Montgomery form; equal keys are
+ * bit-identical, so the result is unique.  An exact LSD radix sort over the canonical bytes that skips every byte position at
+ * which all keys agree: the call reads which positions vary back to the host, so it returns once the kernels before that copy on
+ * `stream` have run.  d_out may equal d_in (in place) but must not overlap it otherwise; n < 2^31; the workspace must not overlap
+ * d_in or d_out. */
+int gmsm_fr_sort_device(int fr_field, const void* d_in, size_t n, void* d_out, void* d_work, void* stream);
+/* evaluateAccumulationPolynomial (vector.go:52-95), in natural order: d_z[0] = 1, d_z[i+1] = d_z[i] (1+beta)(gamma+f[i])
+ * (gamma(1+beta)+t[i]+beta t[i+1]) / ((gamma(1+beta)+h1[i]+beta h1[i+1])(gamma(1+beta)+h2[i]+beta h2[i+1])), zero -> zero
+ * inversion as fr.BatchInvert.  The workspace is gmsm_fr_permutation_workspace_bytes(fr_field, n) bytes (the same scan).  d_z must
+ * not overlap the four inputs, which are left unchanged. */
+int gmsm_fr_plookup_accumulate_device(int fr_field, const void* d_f, const void* d_t, const void* d_h1, const void* d_h2, size_t n,
+                                      const uint64_t* beta, const uint64_t* gamma, void* d_z, void* d_work, void* stream);
+/* the quotient of plookup.ProveLookupVector before its inverse FFT (evaluateNumBitReversed, evaluateZStartsByOneBitReversed,
+ * evaluateZEndsByOneBitReversed, evaluateOverlapH1h2BitReversed and computeQuotientCanonical, vector.go:97-335) from the
+ * bit-reversed coset DIF outputs lz, lh1, lh2, lt, lf on `domain` (the big domain, of size 2s): the four constraint terms folded
+ * with alpha and divided by x^s - 1.  n must equal the domain cardinality; d_out must not overlap the inputs, which are left
+ * unchanged. */
+int gmsm_fft_plookup_numerator_device(gmsm_fft_domain_t* domain, const void* d_lz, const void* d_lh1, const void* d_lh2, const void* d_lt,
+                                      const void* d_lf, size_t n, const uint64_t* beta, const uint64_t* gamma, const uint64_t* alpha,
+                                      void* d_out, void* stream);
+
 /* ---- kzg.ToLagrangeG1 (ecc/bn254/kzg/utils.go:25-64; the same for the other pairing curves): the canonical SRS [tau^i]G in,
  * its Lagrange form [L_i(tau)]G out, by an inverse FFT over G1 points on the device.  Curves: the G1 groups of bn254, bls12-381,
  * bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761 (others: GMSM_EINVAL).  Points are the reference's in-memory G1Affine
