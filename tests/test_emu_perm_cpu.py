@@ -112,8 +112,8 @@ def _perm_case(n, rng, r):
 
 @pytest.mark.parametrize("c", list(FIELDS))
 def test_accumulate_levels(c):
-    """the accumulation polynomial in the bit-reversed layout: one, two and three scan levels at the scan tile of fft.cu
-    (T = 1024, n up to 4T) and at forced small tiles (T = 8 and T = 2: n up to 2^10 reaches four and more levels)"""
+    """the accumulation polynomial in the bit-reversed layout: one and two scan levels at the scan tile of fft.cu
+    (T = 1024, n up to 4T; three need n > T^2) and at forced small tiles (T = 8 and T = 2: n up to 2^10 reaches four and more levels)"""
     cp = _kzg().CURVE_PARAMS[c]
     r = cp.r
     rng = random.Random(17 + FIELDS[c])

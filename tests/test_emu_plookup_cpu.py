@@ -127,7 +127,7 @@ def _lookup_case(n, rng, r):
 
 @pytest.mark.parametrize("c", list(FIELDS))
 def test_accumulate(c):
-    """the accumulation polynomial at the tiles of fft.cu (one to three scan levels) and at forced small tiles, n = 1 ... 2^11; and
+    """the accumulation polynomial at the tiles of fft.cu (one and two scan levels) and at forced small tiles (up to eight), n = 1 ... 2^11; and
     with beta, gamma chosen so that gamma(1 + beta) + h1[i] + beta h1[i + 1] = 0 (the zero -> zero inversion of fr.BatchInvert zeroes
     z past i + 1)"""
     r = _r(c)

@@ -71,7 +71,7 @@ def _accumulate(c, d_t1, d_t2, n, eps):
 @pytest.mark.parametrize("c", CURVES)
 def test_abi_batch_invert_and_accumulate(c):
     """BatchInvert with zeros at the start, the end, in a run and everywhere, across tile boundaries and in place; the accumulation
-    polynomial at n = 1, 2, 2^10, 2^16 (three scan levels) with random eps and eps forced to a t2[k] and a t1[k]; inputs unchanged"""
+    polynomial at n = 1, 2, 2^10, 2^16 (one and two scan levels; three in test_gpu_perm_stress.py) with random eps and eps forced to a t2[k] and a t1[k]; inputs unchanged"""
     kzg = _mods()[0]
     torch = _torch()
     L = _nat().lib()
