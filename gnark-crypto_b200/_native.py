@@ -78,6 +78,8 @@ _SIGNATURES = [
     ("gmsm_g1_to_lagrange_workspace_bytes", sz, [i32, sz]),
     ("gmsm_g1_to_lagrange", i32, [i32, vp, sz, i32, vp]),
     ("gmsm_g1_to_lagrange_device", i32, [i32, vp, sz, vp, vp, vp]),
+    ("gmsm_scale_powers", i32, [i32, vp, sz, vp, vp, i32, vp]),
+    ("gmsm_scale_powers_device", i32, [i32, vp, sz, vp, vp, vp, vp]),
     ("gmsm_test_op", i32, [i32, i32, vp, vp, vp, sz]),
     ("gmsm_test_digits", i32, [i32, i32, vp, sz, vp]),
 ]

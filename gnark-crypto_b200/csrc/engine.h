@@ -151,6 +151,10 @@ struct GroupVTable {
   int (*digits_dump)(const void* d_scalars, size_t n, int c, int nwin, uint32_t* dout);
   int (*batch_scalar_mul)(const void* d_table, const void* d_scalars, size_t n, int c, int nwin, void* d_out, cudaStream_t);
   int (*table_level)(const void* d_in, size_t n, int c, void* d_out, cudaStream_t);   // out[i] = 2^c * in[i]
+  bool (*fr_reduced)(const uint64_t* limbs);   // an fr.Element (Montgomery u64 limbs) below the scalar field's modulus
+  // out[i] = [c r^(start + i)] points[i] for 1 <= n < 2^32 affine points (mpc_kernels.cuh), affine normal form; c, r reduced
+  // Montgomery fr limbs; d_out may equal d_points
+  int (*scale_powers)(const void* d_points, size_t n, const uint64_t* c, const uint64_t* r, uint64_t start, void* d_out, cudaStream_t);
   // kzg.ToLagrangeG1 (lagrange_kernels.cuh) on n = 2^k >= 2 affine points: w_inv = fr.Generator(n)^-1 and n_inv = 1/n as
   // Montgomery fr limbs, d_work holds n extended-Jacobian points.  Null except for the G1 groups of the pairing curves.
   int (*to_lagrange)(const void* d_points, size_t n, const uint64_t* w_inv, const uint64_t* n_inv, void* d_out, void* d_work,

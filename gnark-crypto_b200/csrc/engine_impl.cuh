@@ -6,6 +6,7 @@
 #include "kernels.cuh"
 #include "affine_kernels.cuh"
 #include "lagrange_kernels.cuh"
+#include "mpc_kernels.cuh"
 
 namespace gmsm {
 
@@ -365,13 +366,34 @@ static int run_to_lagrange(const void* d_points, size_t n, const uint64_t* w_inv
   return GMSM_OK;
 }
 
+// out[i] = [c r^(start + i)] points[i], 1 <= n < 2^32 (mpc_kernels.cuh): one launch on st
+template <class G>
+static int run_scale_powers(const void* d_points, size_t n, const uint64_t* c, const uint64_t* r, uint64_t start, void* d_out,
+                            cudaStream_t st) {
+  using A = Affine<typename G::F>;
+  const ScalePowers<G> pw = scale_powers_args<G>(c, r, start);
+  scale_powers_schedule(n, [&](uint64_t threads) {
+    k_scale_powers<G><<<nblk(threads, 128), 128, 0, st>>>(reinterpret_cast<const A*>(d_points), (uint32_t)n, pw, reinterpret_cast<A*>(d_out));
+  });
+  LAUNCH_CHECK();
+  return GMSM_OK;
+}
+
+template <class G>
+static bool fr_reduced(const uint64_t* limbs) {
+  typename G::Fr x;
+  memcpy(x.l, limbs, sizeof(x));
+  return fp_is_reduced(x);
+}
+
 #define GMSM_CURVE_INFO(G) {G::F::N, G::FrParams::BITS, 4 * G::FrParams::N}
 #define GMSM_INSTANTIATE(G, NAME)                                                                  \
   const GroupVTable NAME = {GMSM_CURVE_INFO(G), &run_window_sums<G>, &run_accumulate<G>, &run_bucket_reduce<G>, &run_finalize<G>, &run_generate<G>, \
-                            &test_op_sizes<G>, &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>};
+                            &test_op_sizes<G>, &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>, &fr_reduced<G>, &run_scale_powers<G>};
 // the G1 groups of the seven pairing curves: also kzg.ToLagrangeG1
 #define GMSM_INSTANTIATE_PAIRING_G1(G, NAME)                                                       \
   const GroupVTable NAME = {GMSM_CURVE_INFO(G), &run_window_sums<G>, &run_accumulate<G>, &run_bucket_reduce<G>, &run_finalize<G>, &run_generate<G>, \
-                            &test_op_sizes<G>, &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>, &run_to_lagrange<G>};
+                            &test_op_sizes<G>, &run_test_op<G>, &run_digits_dump<G>, &run_batch_scalar_mul<G>, &run_table_level<G>, &fr_reduced<G>, &run_scale_powers<G>, \
+                            &run_to_lagrange<G>};
 
 }  // namespace gmsm

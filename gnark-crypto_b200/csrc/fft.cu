@@ -65,12 +65,6 @@ Fp<P> host_pow2k(Fp<P> x, int k) {  // x^(2^k)
   for (int i = 0; i < k; i++) x = fp_sqr(x);
   return x;
 }
-template <class P>
-bool host_is_reduced(const Fp<P>& x) {  // x < r: a valid fr.Element
-  for (int i = P::N - 1; i >= 0; i--)
-    if (x.l[i] != P::mod(i)) return x.l[i] < P::mod(i);
-  return false;
-}
 
 struct FrConsts {
   const char* root;   // fr.Generator's rootOfUnity (decimal), generator.go:23
@@ -334,7 +328,7 @@ extern "C" int gmsm_fr_poly_div_x_minus_a_device(int fr_field, const void* d_f, 
     using F = Fp<P>;
     F av;
     memcpy(av.l, a, sizeof(F));
-    if (!host_is_reduced(av)) return set_err(GMSM_EINVAL, "the point is not a reduced fr.Element");
+    if (!fp_is_reduced(av)) return set_err(GMSM_EINVAL, "the point is not a reduced fr.Element");
     constexpr int log_l = poly_log_l<P>(), log_b = poly_log_b<P>();
     if (((n - 1) >> (log_l + log_b)) >= 0x7fffffffull) return set_err(GMSM_EINVAL, "polynomial too large (n = %zu)", n);
     const size_t smem = poly_smem_bytes<P>(log_l, log_b);
@@ -378,7 +372,7 @@ extern "C" int gmsm_fr_poly_fold_device(int fr_field, const void* const* d_polys
     using F = Fp<P>;
     F g;
     memcpy(g.l, gamma, sizeof(F));
-    if (!host_is_reduced(g)) return set_err(GMSM_EINVAL, "gamma is not a reduced fr.Element");
+    if (!fp_is_reduced(g)) return set_err(GMSM_EINVAL, "gamma is not a reduced fr.Element");
     std::vector<uint64_t> len(lens, lens + k);
     const auto launch = poly_fold_launcher<P>(d_out, out_len, stream);
     poly_fold_schedule<P>(reinterpret_cast<const F* const*>(d_polys), len.data(), k, g,
@@ -409,7 +403,7 @@ extern "C" int gmsm_fr_poly_lincomb_device(int fr_field, const void* const* d_po
     std::vector<F> s(k);
     for (size_t i = 0; i < k; i++) {
       memcpy(s[i].l, scalars + i * (fb / 8), sizeof(F));
-      if (!host_is_reduced(s[i])) return set_err(GMSM_EINVAL, "scalar %zu is not a reduced fr.Element", i);
+      if (!fp_is_reduced(s[i])) return set_err(GMSM_EINVAL, "scalar %zu is not a reduced fr.Element", i);
     }
     std::vector<uint64_t> len(lens, lens + k), str(strides, strides + k), off(offsets, offsets + k);
     poly_lincomb_schedule<P>(reinterpret_cast<const F* const*>(d_polys), len.data(), s.data(), str.data(), off.data(), k,
@@ -434,7 +428,7 @@ unsigned perm_inv_tiles(uint64_t n) { return (unsigned)(((n - 1) >> PERM_INV_LOG
 template <class P>
 bool read_reduced(const uint64_t* limbs, Fp<P>* out) {
   memcpy(out->l, limbs, sizeof(Fp<P>));
-  return host_is_reduced(*out);
+  return fp_is_reduced(*out);
 }
 
 }  // namespace

@@ -188,6 +188,14 @@ GMSM_HD void fp_reduce_once(Fp<P>& a, uint32_t carry = 0) {
 #endif
 }
 
+// x < q: a valid (reduced) element
+template <class P>
+GMSM_HD bool fp_is_reduced(const Fp<P>& x) {
+  for (int i = P::N - 1; i >= 0; i--)
+    if (x.l[i] != P::mod(i)) return x.l[i] < P::mod(i);
+  return false;
+}
+
 // fp.Add  (fp/element.go:386-401): a, b < q
 template <class P>
 GMSM_HD Fp<P> fp_add(const Fp<P>& a, const Fp<P>& b) {

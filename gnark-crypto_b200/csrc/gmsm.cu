@@ -1315,6 +1315,63 @@ extern "C" int gmsm_g1_to_lagrange(gmsm_curve_t curve, const uint64_t* points, s
 }
 
 // ------------------------------------------------------------------------------------------
+// mpcsetup: out[i] = [c r^i] points[i] (UpdateMonomialsG1 / G2, the alpha / beta tau^i slices, UpdateValues;
+// ecc/<curve>/mpcsetup/mpcsetup.go), mpc_kernels.cuh
+// ------------------------------------------------------------------------------------------
+// points per chunk of the host entry: bounds its device memory (192 MB for the 12-word groups); the result does not depend on it
+static constexpr size_t SCALE_HOST_CHUNK = (size_t)1 << 20;
+
+// the argument checks of both entry points after n > 0, before any device work
+static int scale_args(int curve, const void* points, size_t n, const uint64_t* c, const uint64_t* r, const void* out) {
+  const GroupVTable* vt = vtable(curve);
+  if (!points || !out || !c || !r) return set_err(GMSM_EINVAL, "null argument");
+  if (!vt->fr_reduced(c)) return set_err(GMSM_EINVAL, "c is not a reduced fr.Element");
+  if (!vt->fr_reduced(r)) return set_err(GMSM_EINVAL, "r is not a reduced fr.Element");
+  const size_t bytes = n * gmsm_affine_bytes((gmsm_curve_t)curve);
+  const uintptr_t p0 = (uintptr_t)points, o0 = (uintptr_t)out;
+  if (p0 != o0 && p0 < o0 + bytes && o0 < p0 + bytes) return set_err(GMSM_EINVAL, "the output must equal the points or not overlap them");
+  return GMSM_OK;
+}
+
+extern "C" int gmsm_scale_powers_device(gmsm_curve_t curve, const void* d_points, size_t n, const uint64_t* c, const uint64_t* r,
+                                        void* d_out, void* stream) {
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  if (n == 0) return GMSM_OK;
+  if (int rc = scale_args(curve, d_points, n, c, r, d_out)) return rc;
+  if (n >= ((size_t)1 << 32)) return set_err(GMSM_EINVAL, "n = %zu points: at most 2^32 - 1 per call", n);
+  if (int rc = set_device_of(d_out)) return rc;
+  return vt->scale_powers(d_points, n, c, r, 0, d_out, (cudaStream_t)stream);
+}
+
+extern "C" int gmsm_scale_powers(gmsm_curve_t curve, const uint64_t* points, size_t n, const uint64_t* c, const uint64_t* r, int device,
+                                 uint64_t* out) {
+  const GroupVTable* vt = vtable(curve);
+  if (!vt) return set_err(GMSM_EINVAL, "unknown curve id %d", (int)curve);
+  if (n == 0) return GMSM_OK;
+  if (int rc = scale_args(curve, points, n, c, r, out)) return rc;
+  if (int rc = use_device(device)) return rc;
+  const size_t ab = gmsm_affine_bytes(curve), len = std::min(n, SCALE_HOST_CHUNK);
+  DevBuf buf;
+  cudaStream_t st = nullptr;
+  if (cudaMalloc(&buf.p, len * ab) != cudaSuccess || cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess)
+    return set_err(GMSM_ENOMEM, "gmsm_scale_powers: device allocation failed");
+  // chunk k starts at index k len: its kernel scales by c r^(k len), so every chunking gives the same points
+  int rc = GMSM_OK;
+  cudaError_t ce = cudaSuccess;
+  for (size_t lo = 0; lo < n && rc == GMSM_OK && ce == cudaSuccess; lo += len) {
+    const size_t m = std::min(len, n - lo);
+    ce = cudaMemcpyAsync(buf.p, points + lo * (ab / 8), m * ab, cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess) rc = vt->scale_powers(buf.p, m, c, r, lo, buf.p, st);
+    if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaMemcpyAsync(out + lo * (ab / 8), buf.p, m * ab, cudaMemcpyDeviceToHost, st);
+    if (ce == cudaSuccess && rc == GMSM_OK) ce = cudaStreamSynchronize(st);
+  }
+  if (ce != cudaSuccess) rc = set_err(GMSM_ECUDA, "gmsm_scale_powers: %s", cudaGetErrorString(ce));
+  cudaStreamDestroy(st);
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------
 // test hooks
 // ------------------------------------------------------------------------------------------
 extern "C" int gmsm_test_op(gmsm_curve_t curve, int op, const uint32_t* a, const uint32_t* b, uint32_t* out, size_t n) {

@@ -53,10 +53,11 @@ GMSM_D XYZZ<F> lag_entry(const XYZZ<F>* tab, uint32_t code) {
 // over fr.Bits / W + 1 windows, so the top window (at most W - 1 bits plus a carry) stays within the table as well.
 // Horner from the top non-zero window: W Jacobian doublings (dbl-2009-l, 2M + 5S) and one extended-Jacobian addition of
 // +-table entry per window (the Horner step of k_finalize); the addition takes the doubling and cancellation branches.
-template <class G>
+// W: ToLagrangeG1's lag_w unless a caller of another shape chooses its own (mpc_kernels.cuh).
+template <class G, int W = lag_w<G>>
 GMSM_D XYZZ<typename G::F> lag_scalar_mul(const XYZZ<typename G::F>& p, const typename G::Fr& s) {
   using F = typename G::F;
-  constexpr int W = lag_w<G>, NWIN = G::FrParams::BITS / W + 1, NT = 1 << (W - 1);
+  constexpr int NWIN = G::FrParams::BITS / W + 1, NT = 1 << (W - 1);
   static_assert(W >= 2 && W <= 7, "the window codes are stored in bytes");
   if (p.is_inf() || s.is_zero()) return XYZZ<F>::inf();
   uint8_t codes[NWIN];

@@ -313,6 +313,23 @@ int gmsm_g1_to_lagrange(gmsm_curve_t curve, const uint64_t* points, size_t n, in
  * gmsm_g1_to_lagrange_workspace_bytes(curve, n) bytes (unused for n = 1). */
 int gmsm_g1_to_lagrange_device(gmsm_curve_t curve, const void* d_points, size_t n, void* d_out, void* d_work, void* stream);
 
+/* ---- mpcsetup (ecc/bn254/mpcsetup/mpcsetup.go; the same for the other pairing curves): the point updates of a trusted-setup
+ * contribution, out[i] = [c r^i] points[i] for i < n, by one variable-base scalar multiplication per point on the device.
+ * UpdateMonomialsG1 / G2 (:365-381) is c = r on points[1:], the alpha tau^i and beta tau^i slices of a powers-of-tau contribution
+ * are c = alpha (beta), the slice loop of UpdateValues (:64-81) is r = 1.  All thirteen groups.  Points are the reference's
+ * in-memory affine points (Montgomery limbs, infinity = zeroes), output in the affine normal form of BatchJacobianToAffineG1;
+ * c and r are fr.Elements (fr.Limbs u64 Montgomery limbs), reduced.  An infinity input stays infinity, as does every point whose
+ * scalar is zero (c = 0; r = 0 past i = 0).  n = 0 is a no-op.  GMSM_EINVAL, before any device work: an unknown group, a null
+ * pointer, an unreduced c or r, an output that overlaps the points without being equal to them. ---- */
+/* host buffers, device `device`; out may equal points (in place).  Works in chunks of 2^20 points (chunk k scaled by
+ * c r^(k 2^20)), so any n fits and the result does not depend on the chunking. */
+int gmsm_scale_powers(gmsm_curve_t curve, const uint64_t* points, size_t n, const uint64_t* c, const uint64_t* r, int device,
+                      uint64_t* out);
+/* device buffers on one device, ordered on `stream` (a cudaStream_t, NULL = default stream); nothing is allocated inside the
+ * call.  d_points is left unmodified unless d_out == d_points (allowed: in place); n < 2^32 (GMSM_EINVAL otherwise). */
+int gmsm_scale_powers_device(gmsm_curve_t curve, const void* d_points, size_t n, const uint64_t* c, const uint64_t* r, void* d_out,
+                             void* stream);
+
 /* ---- 5. test hooks: element-wise device functions, used by tests/ to check the sm_90a field and
  * point arithmetic against the oracle.  a, b, out are HOST arrays of n elements each. ---- */
 enum {
