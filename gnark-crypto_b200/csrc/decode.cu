@@ -11,6 +11,10 @@
 //   bn254 (two spare bits, marshal.go:25-31):      00 uncompressed | 10 compressed, smallest y | 11 largest y | 01 infinity
 //   bls12-381 / bls12-377 / bls24-315 / bls24-317 / bw6-633 / bw6-761 (three bits, :27-34):
 //                                                 000 uncompressed | 010 uncompressed infinity | 100 / 101 compressed | 110 infinity
+// A stream is homogeneous (raw: RawBytes points of 2 * fp.Bytes, else Bytes points of fp.Bytes), so each point is read at a
+// fixed stride and is infinity only under its own kind's flag: 110 in a compressed stream, 010 in a raw one (bn254: none; its
+// RawBytes infinity is the all-zero point, decoded as (0, 0)).  Any other pattern, 010 among compressed points or 110 among
+// raw ones included, is "invalid point encoding": the reference would read such a point at the other kind's length.
 // One thread per point (decode_kernels.cuh); results are the reference's in-memory G1Affine (Montgomery limbs, infinity = zeroes).
 #include <cuda_runtime.h>
 

@@ -169,14 +169,17 @@ k_g1_decode(const uint8_t* __restrict__ bytes, uint32_t n, int raw, int check_cu
   const uint32_t m = b[0] & W::MASK;
   int err = DEC_OK;
   Affine<F> pt = Affine<F>::inf();
-  const bool is_inf = (m == W::INF) || (m == W::UNC_INF);
+  // a stream is homogeneous: raw = 1 holds uncompressed points, raw = 0 compressed ones.  A point is infinity only under its
+  // own stream kind's flag, whose payload is exactly the point's stride (bn254 has no raw infinity flag: its raw infinity is
+  // the all-zero point, which decodes to (0, 0) below); every other pattern is DEC_BAD_FLAGS.
+  const bool is_inf = raw ? (m == W::UNC_INF) : (m == W::INF);
   if (is_inf) {
-    const int len = (m == W::UNC_INF) ? 2 * NB : NB;
+    const int len = raw ? 2 * NB : NB;
     uint32_t any = b[0] & ~W::MASK & 0xFFu;
     for (int k = 1; k < len; k++) any |= b[k];
     if (any) err = DEC_BAD_INFINITY;
   } else if ((raw && m != W::UNC) || (!raw && m != W::SMALL && m != W::LARGE)) {
-    err = DEC_BAD_FLAGS;     // a stream is homogeneous: raw = 1 holds uncompressed points, raw = 0 compressed ones
+    err = DEC_BAD_FLAGS;
   } else {
     const F xc = read_be<P>(b, ~W::MASK & 0xFFu);
     if (!below_modulus(xc)) err = DEC_BAD_ELEMENT;
