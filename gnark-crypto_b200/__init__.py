@@ -10,6 +10,8 @@ Layout:
   dist.py      multi-GPU: one process per GPU, shard points/scalars, all-gather the per-window partials
   fft.py, kzg.py, shplonk.py, fflonk.py, permutation.py, plookup.py, transcript.py: the Fr FFT and the KZG provers; kzg._DevicePoly is
                the one caller of the library's device Fr polynomial entry points
+  iop.py       the Fr layer of a PLONK prover (ecc/<curve>/fr/iop): Polynomial and its forms, Evaluate of a traced expression, the
+               accumulating ratios BuildRatioShuffledVectors / BuildRatioCopyConstraint and DivideByXMinusOne, all on the device
   mpcsetup.py  the point updates of a trusted-setup contribution (UpdateMonomialsG1/G2, ScaleG1/G2) and the linear combinations of
                SameRatioMany (LinearCombinationsG1/G2)
 """

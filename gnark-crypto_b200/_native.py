@@ -75,6 +75,14 @@ _SIGNATURES = [
     ("gmsm_fr_sort_device", i32, [i32, vp, sz, vp, vp, vp]),
     ("gmsm_fr_plookup_accumulate_device", i32, [i32, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]),
     ("gmsm_fft_plookup_numerator_device", i32, [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]),
+    ("gmsm_fr_iop_workspace_bytes", sz, [i32, sz]),
+    ("gmsm_fr_iop_ratio_shuffled_device", i32, [i32, vp, vp, vp, vp, sz, sz, vp, vp, vp, vp]),
+    ("gmsm_fft_iop_ratio_copy_device", i32, [vp, vp, vp, sz, sz, vp, vp, vp, vp, vp, vp]),
+    ("gmsm_fft_iop_lagrange_eval_device", i32, [vp, vp, sz, i32, vp, vp, vp, vp]),
+    ("gmsm_fr_iop_evaluate_device", i32, [i32, vp, sz, sz, vp, sz, vp, vp, vp, sz, sz, i32, vp, vp]),
+    ("gmsm_fr_iop_divide_by_xn_minus_one_device", i32, [i32, vp, sz, u64, i32, vp, sz, vp, vp]),
+    ("gmsm_fr_bit_reverse_device", i32, [i32, vp, sz, vp]),
+    ("gmsm_fr_generator", i32, [i32, u64, vp]),
     ("gmsm_g1_to_lagrange_workspace_bytes", sz, [i32, sz]),
     ("gmsm_g1_to_lagrange", i32, [i32, vp, sz, i32, vp]),
     ("gmsm_g1_to_lagrange_device", i32, [i32, vp, sz, vp, vp, vp]),

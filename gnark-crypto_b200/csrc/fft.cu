@@ -27,6 +27,11 @@
 //   sort.Sort(fr.Vector)                          ecc/bn254/fr/element.go:254 (fr.Element.Cmp)
 //   evaluateAccumulationPolynomial                ecc/bn254/fr/plookup/vector.go:52-95
 //   the quotient numerator and its alpha-fold     ecc/bn254/fr/plookup/vector.go:97-335
+// and the O(n) steps of the iop package (kernels in iop_kernels.cuh; the FFTs are the ones above):
+//   BuildRatioShuffledVectors / BuildRatioCopyConstraint   ecc/bn254/fr/iop/ratios.go:45-246
+//   evalLagrange of Polynomial.Evaluate                    ecc/bn254/fr/iop/polynomial.go:204-241
+//   Evaluate (an interpreted straight-line program)        ecc/bn254/fr/iop/expressions.go:26-73
+//   DivideByXMinusOne                                      ecc/bn254/fr/iop/quotient.go:21-53
 #include <cuda_runtime.h>
 
 #include <cstdio>
@@ -43,6 +48,7 @@ using namespace gmsm;
 #include "poly_kernels.cuh"
 #include "perm_kernels.cuh"
 #include "plookup_kernels.cuh"
+#include "iop_kernels.cuh"
 
 namespace {
 
@@ -636,6 +642,259 @@ extern "C" int gmsm_fft_plookup_numerator_device(gmsm_fft_domain_t* d, const voi
         reinterpret_cast<const F*>(d_lz), reinterpret_cast<const F*>(d_lh1), reinterpret_cast<const F*>(d_lh2), reinterpret_cast<const F*>(d_lt),
         reinterpret_cast<const F*>(d_lf), n, d->logn, k, reinterpret_cast<const F*>(d->d_tw), PERM_INV_LOG_T, reinterpret_cast<F*>(d_out));
     CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+// ---- the O(n) steps of the iop package (ratios.go, polynomial.go:204-241, expressions.go, quotient.go) on device vectors ----
+
+namespace {
+
+int tz64(uint64_t n) {   // bits.TrailingZeros of n > 0
+  int t = 0;
+  while (!((n >> t) & 1ull)) t++;
+  return t;
+}
+
+// the iop workspace: the prefix product's carry levels or the tile sums of the Lagrange evaluation, then one u32 flag
+template <class P>
+size_t iop_flag_offset(uint64_t n) {
+  const size_t scan = poly_levels(n, poly_log_l<P>() + poly_log_b<P>()).work * sizeof(Fp<P>);
+  const size_t sums = (size_t)perm_inv_tiles(n) * sizeof(Fp<P>);
+  return ((scan > sums ? scan : sums) + 15) & ~(size_t)15;
+}
+
+template <class P>
+void iop_prefix(Fp<P>* z, uint64_t n, Fp<P>* work, cudaStream_t st) {
+  constexpr int log_l = poly_log_l<P>(), log_b = poly_log_b<P>();
+  const size_t smem = poly_smem_bytes<P>(log_l, log_b);
+  perm_prefix_schedule<P>(
+      z, n, work, log_l, log_b,
+      [&](const Fp<P>* x, uint64_t m, Fp<P>* heads, uint64_t tiles) {
+        k_perm_prod_heads<P><<<(unsigned)tiles, 1u << log_b, smem, st>>>(x, m, log_l, heads);
+      },
+      [&](Fp<P>* x, uint64_t m, const Fp<P>* carry, uint64_t tiles) {
+        k_perm_prod_write<P><<<(unsigned)tiles, 1u << log_b, smem, st>>>(x, m, log_l, carry);
+      });
+}
+
+// the columns of a ratio builder: non-null, not overlapping the output, at most IOP_MAX_COLUMNS
+template <class P>
+int iop_columns(const void* const* d_cols, const int* bitrev, size_t k, size_t n, const void* d_z, IopColumns<P>* out) {
+  if (k == 0 || k > (size_t)IOP_MAX_COLUMNS) return set_err(GMSM_EINVAL, "%zu polynomials per list (1 to %d are supported)", k, IOP_MAX_COLUMNS);
+  if (!d_cols || !bitrev) return set_err(GMSM_EINVAL, "null column list");
+  const size_t bytes = n * sizeof(Fp<P>);
+  out->k = (int)k;
+  out->bitrev = 0;
+  for (size_t c = 0; c < k; c++) {
+    if (!d_cols[c]) return set_err(GMSM_EINVAL, "polynomial %zu is null", c);
+    if (overlaps(d_z, bytes, d_cols[c], bytes)) return set_err(GMSM_EINVAL, "the output must not overlap polynomial %zu", c);
+    out->p[c] = reinterpret_cast<const Fp<P>*>(d_cols[c]);
+    if (bitrev[c]) out->bitrev |= 1u << c;
+  }
+  return GMSM_OK;
+}
+
+}  // namespace
+
+extern "C" size_t gmsm_fr_iop_workspace_bytes(int fr_field, size_t n) {
+  if (!gmsm_fft_fr_bytes(fr_field) || n == 0) return 0;
+  size_t bytes = 0;
+  with_fr(fr_field, [&](auto tag) {
+    bytes = iop_flag_offset<typename decltype(tag)::type>(n) + 16;
+    return GMSM_OK;
+  });
+  return bytes;
+}
+
+extern "C" int gmsm_fr_iop_ratio_shuffled_device(int fr_field, const void* const* d_num, const int* num_bitrev, const void* const* d_den,
+                                                 const int* den_bitrev, size_t k, size_t n, const uint64_t* beta, void* d_z, void* d_work,
+                                                 void* stream) {
+  if (!gmsm_fft_fr_bytes(fr_field)) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0 || (n & (n - 1))) return set_err(GMSM_EINVAL, "n (%zu) must be a power of 2", n);
+  if (!d_z || !beta || !d_work) return set_err(GMSM_EINVAL, "null output, beta or workspace (gmsm_fr_iop_workspace_bytes)");
+  if (((n - 1) >> PERM_INV_LOG_T) >= 0x7fffffffull) return set_err(GMSM_EINVAL, "vector too large (n = %zu)", n);
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    IopColumns<P> num, den;
+    if (int rc = iop_columns<P>(d_num, num_bitrev, k, n, d_z, &num)) return rc;
+    if (int rc = iop_columns<P>(d_den, den_bitrev, k, n, d_z, &den)) return rc;
+    F b;
+    if (!read_reduced(beta, &b)) return set_err(GMSM_EINVAL, "beta is not a reduced fr.Element");
+    cudaStream_t st = (cudaStream_t)stream;
+    F* z = reinterpret_cast<F*>(d_z);
+    k_iop_ratio_shuffled<P><<<perm_inv_tiles(n), PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), st>>>(num, den, n, tz64(n), b,
+                                                                                                                   PERM_INV_LOG_T, z);
+    iop_prefix<P>(z, n, reinterpret_cast<F*>(d_work), st);
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fft_iop_ratio_copy_device(gmsm_fft_domain_t* d, const void* const* d_cols, const int* bitrev, size_t k, size_t n,
+                                              const int64_t* d_sigma, const uint64_t* beta, const uint64_t* gamma, void* d_z, void* d_work,
+                                              void* stream) {
+  if (!d) return set_err(GMSM_EINVAL, "null domain");
+  if (n != d->n) return set_err(GMSM_EINVAL, "len(a) = %zu must equal the domain cardinality %llu", n, (unsigned long long)d->n);
+  if (!d_z || !beta || !gamma || !d_sigma || !d_work) return set_err(GMSM_EINVAL, "null output, permutation, challenge or workspace");
+  if (((n - 1) >> PERM_INV_LOG_T) >= 0x7fffffffull) return set_err(GMSM_EINVAL, "vector too large (n = %zu)", n);
+  std::lock_guard<std::mutex> lk(d->mu);
+  CK(cudaSetDevice(d->device));
+  return with_fr(d->field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    IopColumns<P> cols;
+    if (int rc = iop_columns<P>(d_cols, bitrev, k, n, d_z, &cols)) return rc;
+    if (overlaps(d_z, n * sizeof(F), d_sigma, k * n * 8)) return set_err(GMSM_EINVAL, "the output must not overlap the permutation");
+    IopCopyConsts<P> kc;
+    F b, g;
+    if (!read_reduced(beta, &b)) return set_err(GMSM_EINVAL, "beta is not a reduced fr.Element");
+    if (!read_reduced(gamma, &kc.gamma)) return set_err(GMSM_EINVAL, "gamma is not a reduced fr.Element");
+    memcpy(g.l, d->consts[3], sizeof(F));
+    for (size_t c = 0; c < k; c++) {
+      kc.p[c] = cols.p[c];
+      kc.bg[c] = b;
+      b = fp_mul(b, g);
+    }
+    kc.bitrev = cols.bitrev;
+    kc.k = (int)k;
+    cudaStream_t st = (cudaStream_t)stream;
+    // an index outside [0, k n) (a panic in the reference) is refused before the output is written: one flag read back
+    uint32_t* flag = reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(d_work) + iop_flag_offset<P>(n));
+    CK(cudaMemsetAsync(flag, 0, 4, st));
+    const uint64_t m = (uint64_t)k * n;
+    k_iop_check_sigma<<<(unsigned)std::min<uint64_t>((m + 255) / 256, GMSM_NUM_SMS * 32u), 256, 0, st>>>(d_sigma, m, (int64_t)m, flag);
+    uint32_t bad = 0;
+    CK(cudaMemcpyAsync(&bad, flag, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (bad) return set_err(GMSM_EINVAL, "the permutation has an entry outside [0, %llu)", (unsigned long long)m);
+    F* z = reinterpret_cast<F*>(d_z);
+    k_iop_ratio_copy<P><<<perm_inv_tiles(n), PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), st>>>(
+        kc, d_sigma, n, d->logn, reinterpret_cast<const F*>(d->d_tw), PERM_INV_LOG_T, z);
+    iop_prefix<P>(z, n, reinterpret_cast<F*>(d_work), st);
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fft_iop_lagrange_eval_device(gmsm_fft_domain_t* d, const void* d_c, size_t n, int bitrev, const uint64_t* x,
+                                                 void* d_out, void* d_work, void* stream) {
+  if (!d) return set_err(GMSM_EINVAL, "null domain");
+  if (n != d->n) return set_err(GMSM_EINVAL, "len(a) = %zu must equal the domain cardinality %llu", n, (unsigned long long)d->n);
+  if (!d_c || !x || !d_out || !d_work) return set_err(GMSM_EINVAL, "null vector, point, output or workspace");
+  if (((n - 1) >> PERM_INV_LOG_T) >= 0x7fffffffull) return set_err(GMSM_EINVAL, "vector too large (n = %zu)", n);
+  std::lock_guard<std::mutex> lk(d->mu);
+  CK(cudaSetDevice(d->device));
+  return with_fr(d->field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    F xv, ci;
+    if (!read_reduced(x, &xv)) return set_err(GMSM_EINVAL, "the point is not a reduced fr.Element");
+    memcpy(ci.l, d->consts[2], sizeof(F));
+    const F scale = fp_mul(fp_sub(host_pow2k(xv, d->logn), F::one()), ci);   // (x^n - 1) / n
+    cudaStream_t st = (cudaStream_t)stream;
+    F* partial = reinterpret_cast<F*>(d_work);
+    const unsigned tiles = perm_inv_tiles(n);
+    k_iop_lagrange_terms<P><<<tiles, PERM_INV_THREADS, perm_inv_smem_bytes<P>(PERM_INV_LOG_T), st>>>(
+        reinterpret_cast<const F*>(d_c), n, d->logn, bitrev, xv, reinterpret_cast<const F*>(d->d_tw), PERM_INV_LOG_T, partial);
+    k_iop_sum<P><<<1, 256, 256 * sizeof(F), st>>>(partial, tiles, scale, reinterpret_cast<F*>(d_out));
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fr_iop_evaluate_device(int fr_field, const uint32_t* code, size_t len, size_t out_reg, const uint64_t* consts,
+                                           size_t nconsts, const void* const* d_inputs, const uint64_t* offsets, const int* bitrev, size_t m,
+                                           size_t n, int out_bitrev, void* d_r, void* stream) {
+  const size_t fb = gmsm_fft_fr_bytes(fr_field);
+  if (!fb) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0) return set_err(GMSM_EINVAL, "empty vector (n = 0)");
+  if (len == 0 || len > (size_t)IOP_MAX_PROGRAM) return set_err(GMSM_EINVAL, "program of %zu instructions (1 to %d)", len, IOP_MAX_PROGRAM);
+  if (out_reg >= (size_t)IOP_MAX_REGISTERS) return set_err(GMSM_EINVAL, "result register %zu (at most %d registers)", out_reg, IOP_MAX_REGISTERS);
+  if (nconsts > (size_t)IOP_MAX_CONSTS) return set_err(GMSM_EINVAL, "%zu constants (at most %d)", nconsts, IOP_MAX_CONSTS);
+  if (m > (size_t)IOP_MAX_INPUTS) return set_err(GMSM_EINVAL, "%zu inputs (at most %d)", m, IOP_MAX_INPUTS);
+  if (!code || !d_r || (nconsts && !consts) || (m && (!d_inputs || !offsets || !bitrev))) return set_err(GMSM_EINVAL, "null argument");
+  for (size_t pc = 0; pc < len; pc++) {
+    const uint32_t w = code[pc], op = w & 0xff, dst = (w >> 8) & 0xff, a = (w >> 16) & 0xff, b = w >> 24;
+    const bool ok = dst < (uint32_t)IOP_MAX_REGISTERS &&
+                    (op == IOP_OP_INPUT ? a < m : op == IOP_OP_CONST ? a < nconsts : op == IOP_OP_INDEX ? true
+                     : op == IOP_OP_NEG ? a < (uint32_t)IOP_MAX_REGISTERS
+                     : op <= IOP_OP_MUL && a < (uint32_t)IOP_MAX_REGISTERS && b < (uint32_t)IOP_MAX_REGISTERS);
+    if (!ok) return set_err(GMSM_EINVAL, "invalid instruction %zu (0x%08x)", pc, w);
+  }
+  IopInputs in{};
+  in.m = (int)m;
+  for (size_t j = 0; j < m; j++) {
+    if (!d_inputs[j]) return set_err(GMSM_EINVAL, "input %zu is null", j);
+    if (offsets[j] >= n) return set_err(GMSM_EINVAL, "offset of input %zu is not below n", j);
+    if (overlaps(d_r, n * fb, d_inputs[j], n * fb)) return set_err(GMSM_EINVAL, "the result must not overlap input %zu", j);
+    in.p[j] = d_inputs[j];
+    in.off[j] = offsets[j];
+    if (bitrev[j]) in.bitrev |= 1u << j;
+  }
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    IopProgram<P> prog;
+    memcpy(prog.code, code, len * 4);
+    prog.len = (int)len;
+    prog.out = (int)out_reg;
+    for (size_t c = 0; c < nconsts; c++)
+      if (!read_reduced(consts + c * (fb / 8), &prog.consts[c])) return set_err(GMSM_EINVAL, "constant %zu is not a reduced fr.Element", c);
+    k_iop_evaluate<P><<<(unsigned)std::min<uint64_t>((n + 255) / 256, GMSM_NUM_SMS * 32u), 256, 0, (cudaStream_t)stream>>>(
+        prog, in, n, tz64(n), out_bitrev, reinterpret_cast<F*>(d_r));
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fr_iop_divide_by_xn_minus_one_device(int fr_field, const void* d_a, size_t n, uint64_t offset, int bitrev,
+                                                         const uint64_t* inv, size_t rho, void* d_out, void* stream) {
+  const size_t fb = gmsm_fft_fr_bytes(fr_field);
+  if (!fb) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0 || (n & (n - 1))) return set_err(GMSM_EINVAL, "n (%zu) must be a power of 2", n);
+  if (rho == 0 || (rho & (rho - 1)) || rho > (size_t)IOP_MAX_RHO) return set_err(GMSM_EINVAL, "rho (%zu) must be a power of 2 up to %d", rho, IOP_MAX_RHO);
+  if (!d_a || !d_out || !inv) return set_err(GMSM_EINVAL, "null vector or inverse table");
+  if (offset >= n) return set_err(GMSM_EINVAL, "offset is not below n");
+  if (overlaps(d_a, n * fb, d_out, n * fb)) return set_err(GMSM_EINVAL, "the output must not overlap the input");
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    using F = Fp<P>;
+    IopXnInv<P> k;
+    k.rho = (uint32_t)rho;
+    for (size_t j = 0; j < rho; j++)
+      if (!read_reduced(inv + j * (fb / 8), &k.inv[j])) return set_err(GMSM_EINVAL, "inverse %zu is not a reduced fr.Element", j);
+    k_iop_div_xn_minus_one<P><<<(unsigned)std::min<uint64_t>((n + 255) / 256, GMSM_NUM_SMS * 32u), 256, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<const F*>(d_a), n, tz64(n), offset, bitrev, k, reinterpret_cast<F*>(d_out));
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fr_bit_reverse_device(int fr_field, void* d_a, size_t n, void* stream) {
+  if (!gmsm_fft_fr_bytes(fr_field)) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (n == 0 || (n & (n - 1))) return set_err(GMSM_EINVAL, "n (%zu) must be a power of 2", n);
+  if (!d_a) return set_err(GMSM_EINVAL, "null vector");
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    k_fft_bit_reverse<P><<<(unsigned)std::min<uint64_t>((n + 255) / 256, GMSM_NUM_SMS * 32u), 256, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<Fp<P>*>(d_a), n, tz64(n));
+    CK(cudaGetLastError());
+    return GMSM_OK;
+  });
+}
+
+extern "C" int gmsm_fr_generator(int fr_field, uint64_t m, uint64_t* out) {
+  const FrConsts* fcp = fr_consts(fr_field);
+  if (!fcp) return set_err(GMSM_EINVAL, "unknown scalar field %d", fr_field);
+  if (!out) return set_err(GMSM_EINVAL, "null output");
+  int logn = 0;
+  if (int rc = domain_log(*fcp, m, &logn)) return rc;
+  return with_fr(fr_field, [&](auto tag) -> int {
+    using P = typename decltype(tag)::type;
+    const Fp<P> g = host_pow2k(host_from_decimal<P>(fcp->root), fcp->max_order - logn);
+    memcpy(out, g.l, sizeof(Fp<P>));
     return GMSM_OK;
   });
 }

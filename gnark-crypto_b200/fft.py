@@ -23,6 +23,7 @@ class Domain:
         if curve not in CURVE_PARAMS:
             raise MultiExpError("unknown curve %r (FFT over Fr: %s)" % (curve, ", ".join(CURVE_PARAMS)))
         fr_id = CURVE_PARAMS[curve].fr_id
+        self.curve = curve
         self.words = int(L.gmsm_fft_fr_bytes(fr_id)) // 8
         sp = None
         if shift is not None:

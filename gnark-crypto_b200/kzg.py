@@ -248,6 +248,61 @@ class _DevicePoly:
             domain._h, d_lz.data_ptr(), d_lh1.data_ptr(), d_lh2.data_ptr(), d_lt.data_ptr(), d_lf.data_ptr(), domain.Cardinality,
             beta.ctypes.data, gamma.ctypes.data, alpha.ctypes.data, d_out.data_ptr(), self.stream))
 
+    def bit_reverse(self, d_a, n: int):
+        """fft.BitReverse of d_a in place (n a power of two)"""
+        _check(_native.lib().gmsm_fr_bit_reverse_device(self.field, d_a.data_ptr(), n, self.stream))
+
+    # the iop package (iop.py): every call takes the workspace of gmsm_fr_iop_workspace_bytes for n elements, allocated once per size
+    def _iop_work(self, n: int):
+        ws = int(_native.lib().gmsm_fr_iop_workspace_bytes(self.field, n))
+        if getattr(self, "_iop_ws", None) is None or self._iop_ws.numel() * 8 < ws:
+            self._iop_ws = self.torch.empty((ws + 7) // 8, dtype=self.torch.int64, device=self.dev)
+        return self._iop_ws
+
+    def iop_ratio_shuffled(self, d_num, num_bitrev, d_den, den_bitrev, n: int, beta: np.ndarray, d_z):
+        """d_z = the accumulating ratio of BuildRatioShuffledVectors in Lagrange Regular form (inputs already in Lagrange form)"""
+        k = len(d_num)
+        num = (ctypes.c_void_p * k)(*[d.data_ptr() for d in d_num])
+        den = (ctypes.c_void_p * k)(*[d.data_ptr() for d in d_den])
+        nb, db = (ctypes.c_int * k)(*num_bitrev), (ctypes.c_int * k)(*den_bitrev)
+        work = self._iop_work(n)
+        _check(_native.lib().gmsm_fr_iop_ratio_shuffled_device(self.field, num, nb, den, db, k, n, beta.ctypes.data, d_z.data_ptr(),
+                                                               work.data_ptr(), self.stream))
+
+    def iop_ratio_copy(self, domain, d_cols, bitrev, d_sigma, beta: np.ndarray, gamma: np.ndarray, d_z):
+        """d_z = the accumulating ratio of BuildRatioCopyConstraint in Lagrange Regular form; d_sigma: int64 tensor of k n entries.
+        Returns once the permutation has been checked."""
+        k, n = len(d_cols), domain.Cardinality
+        cols = (ctypes.c_void_p * k)(*[d.data_ptr() for d in d_cols])
+        br = (ctypes.c_int * k)(*bitrev)
+        work = self._iop_work(n)
+        _check(_native.lib().gmsm_fft_iop_ratio_copy_device(domain._h, cols, br, k, n, d_sigma.data_ptr(), beta.ctypes.data, gamma.ctypes.data,
+                                                            d_z.data_ptr(), work.data_ptr(), self.stream))
+
+    def iop_lagrange_eval(self, domain, d_c, bitrev: bool, x: np.ndarray, d_out):
+        """d_out = evalLagrange of d_c (Lagrange basis on `domain`) at x"""
+        work = self._iop_work(domain.Cardinality)
+        _check(_native.lib().gmsm_fft_iop_lagrange_eval_device(domain._h, d_c.data_ptr(), domain.Cardinality, 1 if bitrev else 0, x.ctypes.data,
+                                                               d_out.data_ptr(), work.data_ptr(), self.stream))
+
+    def iop_evaluate(self, code: np.ndarray, out_reg: int, consts: np.ndarray, d_inputs, offsets, bitrev, n: int, out_bitrev: bool, d_r):
+        """d_r = the straight-line program `code` over the inputs, one value per position (iop.Evaluate)"""
+        m = len(d_inputs)
+        ins = (ctypes.c_void_p * max(m, 1))(*[d.data_ptr() for d in d_inputs])
+        off = np.array(list(offsets) or [0], dtype=np.uint64)
+        br = (ctypes.c_int * max(m, 1))(*(list(bitrev) or [0]))
+        code = np.ascontiguousarray(code, dtype=np.uint32)
+        consts = np.ascontiguousarray(consts, dtype=np.uint64)
+        _check(_native.lib().gmsm_fr_iop_evaluate_device(self.field, code.ctypes.data, code.shape[0], out_reg, consts.ctypes.data,
+                                                         consts.shape[0], ins, off.ctypes.data, br, m, n, 1 if out_bitrev else 0,
+                                                         d_r.data_ptr(), self.stream))
+
+    def iop_divide_by_xn_minus_one(self, d_a, n: int, offset: int, bitrev: bool, inv: np.ndarray, d_out):
+        """d_out[rev(i)] = a.GetCoeff(i) inv[i mod rho] (DivideByXMinusOne before its inverse FFT)"""
+        inv = np.ascontiguousarray(inv, dtype=np.uint64)
+        _check(_native.lib().gmsm_fr_iop_divide_by_xn_minus_one_device(self.field, d_a.data_ptr(), n, offset, 1 if bitrev else 0,
+                                                                       inv.ctypes.data, inv.shape[0], d_out.data_ptr(), self.stream))
+
 
 @dataclass
 class OpeningProof:

@@ -298,6 +298,49 @@ int gmsm_fft_plookup_numerator_device(gmsm_fft_domain_t* domain, const void* d_l
                                       const void* d_lf, size_t n, const uint64_t* beta, const uint64_t* gamma, const uint64_t* alpha,
                                       void* d_out, void* stream);
 
+/* ---- the O(n) steps of the iop package (ecc/bn254/fr/iop: ratios.go, polynomial.go, expressions.go, quotient.go; the same for
+ * the other six scalar fields), with the conventions of the blocks above.  Limits, refused with GMSM_EINVAL: at most 32
+ * polynomials per list of a ratio builder; an Evaluate program of at most 256 instructions over at most 16 registers (live
+ * values), 32 constants and 32 inputs; a DivideByXMinusOne ratio rho = len / size that is a power of two up to 64. ---- */
+/* bytes of device workspace every gmsm_*_iop_* call with a workspace needs for n elements (0 for n = 0 or an unknown field) */
+size_t gmsm_fr_iop_workspace_bytes(int fr_field, size_t n);
+/* BuildRatioShuffledVectors after ToLagrange (ratios.go:78-119): d_z[k] = prod_{i<k} prod_c (beta - num_c[i]) / prod_c (beta -
+ * den_c[i]) in natural order (Lagrange, Regular), d_z[0] = 1, zero -> zero inversion (every d_z[k] past the first zero denominator
+ * is zero, as in the reference).  k columns per list; column c is read at i, or at its bit reversal when *_bitrev[c] != 0.  n a
+ * power of two; d_z must not overlap a column, which are left unchanged. */
+int gmsm_fr_iop_ratio_shuffled_device(int fr_field, const void* const* d_num, const int* num_bitrev, const void* const* d_den,
+                                      const int* den_bitrev, size_t k, size_t n, const uint64_t* beta, void* d_z, void* d_work,
+                                      void* stream);
+/* BuildRatioCopyConstraint after ToLagrange (ratios.go:165-238): d_z[k] = prod_{i<k} prod_c (P_c[i] + beta g^c w^i + gamma) /
+ * prod_c (P_c[i] + beta ID[sigma[c n + i]] + gamma), ID[s] = g^(s / n) w^(s mod n), w and g = FrMultiplicativeGen of `domain`, in
+ * natural order, d_z[0] = 1, zero -> zero inversion.  d_sigma: k n int64 entries on the device.  An entry outside [0, k n) is
+ * refused before d_z is written: the call reads one flag back, so it returns once the work before it on `stream` has run.  n must
+ * equal the domain cardinality; d_z must not overlap a column or sigma. */
+int gmsm_fft_iop_ratio_copy_device(gmsm_fft_domain_t* domain, const void* const* d_cols, const int* bitrev, size_t k, size_t n,
+                                   const int64_t* d_sigma, const uint64_t* beta, const uint64_t* gamma, void* d_z, void* d_work,
+                                   void* stream);
+/* evalLagrange (polynomial.go:204-241): *d_out = (x^n - 1) / n sum_i w^i / (x - w^i) c[idx(i)], idx(i) = i or its bit reversal
+ * (bitrev != 0), w the generator of `domain`; zero for x on the domain, as in the reference.  n must equal the domain cardinality. */
+int gmsm_fft_iop_lagrange_eval_device(gmsm_fft_domain_t* domain, const void* d_c, size_t n, int bitrev, const uint64_t* x, void* d_out,
+                                      void* d_work, void* stream);
+/* Evaluate (expressions.go:26-73) of a straight-line program: d_r[idx(i)] = f(i, x_0.GetCoeff(i), ...) for i < n, idx(i) = i or
+ * Reverse64(i) >> (64 - TrailingZeros(n)) (out_bitrev != 0).  Input j is read at (i + offsets[j]) mod n, bit-reversed the same way
+ * when bitrev[j] != 0 (offsets[j] = (len / size) shift mod n).  Instruction word: op | dst << 8 | a << 16 | b << 24, op 0 input a,
+ * 1 constant a, 2 the index i, 3 add, 4 sub, 5 mul (registers a, b), 6 negate (register a); register out_reg holds f.  Constants:
+ * nconsts reduced Montgomery elements.  d_r must not overlap an input. */
+int gmsm_fr_iop_evaluate_device(int fr_field, const uint32_t* code, size_t len, size_t out_reg, const uint64_t* consts, size_t nconsts,
+                                const void* const* d_inputs, const uint64_t* offsets, const int* bitrev, size_t m, size_t n, int out_bitrev,
+                                void* d_r, void* stream);
+/* the elementwise step of DivideByXMinusOne (quotient.go:40-47): d_out[rev(i)] = a[(i + offset) mod n, bit-reversed when bitrev !=
+ * 0] inv[i mod rho] for i < n, n a power of two; inv: rho reduced Montgomery elements.  d_out must not overlap d_a. */
+int gmsm_fr_iop_divide_by_xn_minus_one_device(int fr_field, const void* d_a, size_t n, uint64_t offset, int bitrev, const uint64_t* inv,
+                                              size_t rho, void* d_out, void* stream);
+/* fft.BitReverse (bitreverse.go:17-42) of d_a in place, n a power of two, without a domain */
+int gmsm_fr_bit_reverse_device(int fr_field, void* d_a, size_t n, void* stream);
+/* fr.Generator(m) (generator.go:18-36): the root of unity of order ecc.NextPowerOfTwo(m), host only, into out (fr.Limbs Montgomery
+ * limbs); GMSM_EINVAL past the field's 2-adicity */
+int gmsm_fr_generator(int fr_field, uint64_t m, uint64_t* out);
+
 /* ---- kzg.ToLagrangeG1 (ecc/bn254/kzg/utils.go:25-64; the same for the other pairing curves): the canonical SRS [tau^i]G in,
  * its Lagrange form [L_i(tau)]G out, by an inverse FFT over G1 points on the device.  Curves: the G1 groups of bn254, bls12-381,
  * bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761 (others: GMSM_EINVAL).  Points are the reference's in-memory G1Affine
