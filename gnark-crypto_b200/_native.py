@@ -54,6 +54,10 @@ _SIGNATURES = [
     ("gmsm_batch_scalar_mul", i32, [i32, vp, vp, sz, vp]),
     ("gmsm_g1_decode", i32, [i32, vp, sz, i32, i32, vp]),
     ("gmsm_g1_decode_device", i32, [i32, vp, sz, i32, i32, vp, vp, vp]),
+    ("gmsm_g2_decode", i32, [i32, vp, sz, i32, i32, vp]),
+    ("gmsm_g2_decode_device", i32, [i32, vp, sz, i32, i32, vp, vp, vp]),
+    ("gmsm_points_encode", i32, [i32, vp, sz, i32, vp]),
+    ("gmsm_points_encode_device", i32, [i32, vp, sz, i32, vp, vp]),
     ("gmsm_fft_fr_bytes", sz, [i32]),
     ("gmsm_fft_domain_create", vp, [i32, u64, vp, i32]),
     ("gmsm_fft_domain_free", None, [vp]),

@@ -106,6 +106,23 @@ class ProvingKey:
     def close(self):
         self._bases.close()
 
+    def WriteTo(self, w) -> int:
+        """ProvingKey.WriteTo (kzg/marshal.go:16-33): pk.G1 as a compressed []G1Affine slice, encoded on the GPU.  Returns the
+        bytes written."""
+        return write_points(w, self.curve, self.G1, raw=False)
+
+    def WriteRawTo(self, w) -> int:
+        """ProvingKey.WriteRawTo: the same without point compression (RawEncoding)"""
+        return write_points(w, self.curve, self.G1, raw=True)
+
+    @classmethod
+    def UnsafeReadFrom(cls, curve: str, r, device: int = 0):
+        """ProvingKey.UnsafeReadFrom (kzg/marshal.go:140-160): a []G1Affine slice decoded on the GPU without subgroup (or
+        on-curve) checks -> (ProvingKey with the bases resident on `device`, bytes read)"""
+        pts, nbytes = _read_points(r, _g1_name(curve), False, None)
+        return cls(curve, pts, device), nbytes
+
+
 
 def new_srs_g1(curve: str, size: int, alpha: int, generator: np.ndarray, r_modulus: int, encode_scalars) -> np.ndarray:
     """G1 side of kzg.NewSRS (kzg.go:100-135): [1, alpha, alpha^2, ...] * G via BatchScalarMultiplicationG1.
@@ -616,6 +633,176 @@ def decode_g1_points(curve: str, data: bytes, n: int, raw: bool = False, check_o
     out = np.zeros((n, words), dtype=np.uint64)
     _check(_native.lib().gmsm_g1_decode(g.id, buf.ctypes.data, n, 1 if raw else 0, 1 if check_on_curve else 0, out.ctypes.data))
     return out
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# bulk point (de)serialisation on the GPU (csrc/decode.cu): G2Affine.setBytes, and G1Affine / G2Affine Bytes and RawBytes
+# (marshal.go:801-846, :1051-1216), with the slice framing of Encoder / Decoder (a big-endian uint32 count, then the points,
+# marshal.go:220-350, :533-580)
+# ----------------------------------------------------------------------------------------------------------------
+def _g2_group(curve: str):
+    """the Group of a curve's G2 (named with or without "_g2"); ValueError for the bls24 curves, whose G2 is over Fp4"""
+    name = curve if curve.endswith("_g2") else curve + "_g2"
+    if _curve(name) not in CURVE_PARAMS:
+        raise ValueError("unknown pairing curve %r" % curve)
+    if name not in GROUPS:
+        raise ValueError("%s has no G2 in this engine (its G2 is over Fp4)" % _curve(name))
+    return GROUPS[name]
+
+
+def _point_group(group: str):
+    """the Group of a G1 or G2 group name of a pairing curve ("bn254_g1", "bls12381_g2", ...)"""
+    if group.endswith("_g2"):
+        return _g2_group(group)
+    if _curve(group) not in CURVE_PARAMS:
+        raise ValueError("not a pairing curve: %r" % group)
+    return GROUPS[_g1_name(group)]
+
+
+def _point_bytes(g, raw: bool) -> int:
+    """bytes of one encoded point: a coordinate (Bytes) or two (RawBytes)"""
+    return (2 if raw else 1) * 8 * g.words
+
+
+def _decode(fn_host: str, fn_dev: str, g, data, n: int, raw: bool, check_on_curve: bool):
+    words = 2 * g.words
+    per = _point_bytes(g, raw)
+    L = _native.lib()
+    if _is_device(data):
+        import torch
+
+        if not data.is_cuda or data.dtype != torch.uint8 or not data.is_contiguous():
+            raise ValueError("device bytes must be a contiguous torch.uint8 CUDA tensor")
+        if data.numel() < n * per:
+            raise EOFError("short buffer")
+        out = torch.empty(n * words, dtype=torch.int64, device=data.device)
+        err = torch.empty(1, dtype=torch.int64, device=data.device)
+        with torch.cuda.device(data.device):
+            _check(getattr(L, fn_dev)(g.id, data.data_ptr(), n, 1 if raw else 0, 1 if check_on_curve else 0, out.data_ptr(),
+                                      err.data_ptr(), _stream(data.device)))
+            first = int(err.cpu().numpy().view(np.uint64)[0])
+        if first != (1 << 64) - 1:
+            raise MultiExpError("point %d: %s" % (first >> 8, _DECODE_MESSAGES.get(first & 0xFF, "decode error")))
+        return out.view(n, words)
+    if len(data) < n * per:
+        raise EOFError("short buffer")      # io.ErrShortBuffer
+    buf = np.frombuffer(data, dtype=np.uint8, count=n * per)
+    out = np.zeros((n, words), dtype=np.uint64)
+    _check(getattr(L, fn_host)(g.id, buf.ctypes.data, n, 1 if raw else 0, 1 if check_on_curve else 0, out.ctypes.data))
+    return out
+
+
+# the decoder's error codes (decode_kernels.cuh) -> the reference's messages, for the device entry's first-error word
+_DECODE_MESSAGES = {1: "invalid infinity point encoding", 2: "invalid fp.Element encoding",
+                    3: "invalid compressed coordinate: square root doesn't exist", 4: "invalid point: subgroup check failed",
+                    5: "invalid point encoding"}
+
+
+def decode_g2_points(curve: str, data, n: int, raw: bool = False, check_on_curve: bool = True):
+    """bulk G2Affine.setBytes without the subgroup check on the GPU (gmsm_g2_decode): n points of a homogeneous stream -> (n,
+    words) uint64 in Go memory layout ({A0, A1} per Fp2 coordinate).  `data` may be a contiguous torch.uint8 CUDA tensor: the
+    points are then decoded on its device, on the current stream, into a torch.int64 tensor (n, words).  Raises MultiExpError
+    with the reference's message and the index of the first invalid point; ValueError for bls24-315 / bls24-317."""
+    g = _g2_group(curve)
+    return _decode("gmsm_g2_decode", "gmsm_g2_decode_device", g, data, n, raw, check_on_curve)
+
+
+def _encode(g, points, raw: bool):
+    words = 2 * g.words
+    per = _point_bytes(g, raw)
+    L = _native.lib()
+    if _is_device(points):
+        import torch
+
+        if not points.is_cuda or points.dtype != torch.int64 or not points.is_contiguous() or points.numel() % words:
+            raise ValueError("device points must be a contiguous torch.int64 CUDA tensor of (n, %d) words" % words)
+        n = points.numel() // words
+        out = torch.empty(max(n * per, 4), dtype=torch.uint8, device=points.device)
+        with torch.cuda.device(points.device):
+            _check(L.gmsm_points_encode_device(g.id, points.data_ptr(), n, 1 if raw else 0, out.data_ptr(), _stream(points.device)))
+        return out[:n * per]
+    pts = np.ascontiguousarray(points, dtype=np.uint64).reshape(-1, words)
+    out = np.empty(max(pts.shape[0] * per, 1), dtype=np.uint8)
+    _check(L.gmsm_points_encode(g.id, pts.ctypes.data, pts.shape[0], 1 if raw else 0, out.ctypes.data))
+    return out[:pts.shape[0] * per].tobytes()
+
+
+def encode_g1_points(curve: str, points, raw: bool = False):
+    """G1Affine.Bytes (raw=False) or RawBytes (raw=True) of every point, on the GPU (gmsm_points_encode): (n, words) uint64 in Go
+    memory layout -> the n encodings back to back (what Encoder writes after the slice length).  A torch.int64 CUDA tensor is
+    encoded on its device, on the current stream, into a torch.uint8 tensor."""
+    return _encode(_point_group(_g1_name(curve)), points, raw)
+
+
+def encode_g2_points(curve: str, points, raw: bool = False):
+    """the G2 twin of encode_g1_points (wire order X.A1 || X.A0 (|| Y.A1 || Y.A0)); ValueError for bls24-315 / bls24-317"""
+    return _encode(_g2_group(curve), points, raw)
+
+
+def write_points(w, group: str, points, raw: bool = False) -> int:
+    """Encoder.Encode of a []G1Affine / []G2Affine (RawEncoding when raw): big-endian uint32 count, then the encoded points.
+    `group`: "<curve>_g1" or "<curve>_g2".  Returns the bytes written."""
+    g = _point_group(group)
+    words = 2 * g.words
+    n = (points.numel() if _is_device(points) else np.asarray(points).size) // words
+    if n >= 1 << 32:
+        raise ValueError("too many points for a uint32 slice length")
+    body = _encode(g, points, raw)
+    if _is_device(body):
+        body = body.cpu().numpy().tobytes()
+    w.write(struct.pack(">I", n))
+    w.write(body)
+    return 4 + len(body)
+
+
+def read_points(r, group: str, check_on_curve: bool = False, device=None):
+    """Decoder.Decode of a []G1Affine / []G2Affine with NoSubgroupChecks: a big-endian uint32 count, then the points, whose
+    kind (Bytes or RawBytes) is read from the first point's flags; the stream must be homogeneous (a point of the other kind is
+    "invalid point encoding").  check_on_curve=True also checks raw points against the curve equation, which the reference's
+    NoSubgroupChecks path skips.  -> (n, words) uint64 in Go memory layout (device=None), else decoded on cuda:device into a
+    torch.int64 tensor (the bytes are uploaded once)."""
+    return _read_points(r, group, check_on_curve, device)[0]
+
+
+def _read_points(r, group: str, check_on_curve: bool, device):
+    """read_points -> (points, bytes read)"""
+    g = _point_group(group)
+    hdr = r.read(4)
+    if len(hdr) != 4:
+        raise EOFError("unexpected EOF")
+    (n,) = struct.unpack(">I", hdr)
+    if n == 0:
+        if device is not None:
+            import torch
+
+            return torch.empty((0, 2 * g.words), dtype=torch.int64, device=torch.device("cuda", device)), 4
+        return np.zeros((0, 2 * g.words), dtype=np.uint64), 4
+    first = r.read(1)
+    if len(first) != 1:
+        raise EOFError("unexpected EOF")
+    f = _params(g.curve).flags
+
+    def is_raw(byte: int) -> bool:       # !isCompressed (marshal.go:409-418)
+        m = byte & f["mask"]
+        return m == f["unc"] or (f["unc_inf"] is not None and m == f["unc_inf"])
+
+    raw = is_raw(first[0])
+    per = _point_bytes(g, raw)
+    rest = r.read(n * per - 1)
+    data = first + rest
+    if len(data) != n * per:
+        # a raw stream holding compressed points is shorter than n raw strides: name the first point of the other kind, as the
+        # decoder does for a stream of the right length, before calling the stream short
+        for i in range(len(data) // per):
+            if is_raw(data[i * per]) != raw:
+                raise MultiExpError("point %d: invalid point encoding" % i)
+        raise EOFError("unexpected EOF")
+    fns = ("gmsm_g2_decode", "gmsm_g2_decode_device") if group.endswith("_g2") else ("gmsm_g1_decode", "gmsm_g1_decode_device")
+    if device is not None:
+        import torch
+
+        data = torch.frombuffer(bytearray(data), dtype=torch.uint8).to(torch.device("cuda", device))
+    return _decode(fns[0], fns[1], g, data, n, raw, check_on_curve), 4 + n * per
 
 
 def ToLagrangeG1(coeffs, curve: str, device: int = 0):

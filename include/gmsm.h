@@ -195,6 +195,23 @@ int gmsm_g1_decode(gmsm_curve_t curve, const uint8_t* bytes, size_t n, int raw, 
 /* device buffers; *d_first_error (8 bytes, device) = (index << 8 | code) of the first bad point, all-ones if none */
 int gmsm_g1_decode_device(gmsm_curve_t curve, const void* d_bytes, size_t n, int raw, int check_on_curve, void* d_points,
                           void* d_first_error, void* stream);
+/* G2Affine.setBytes without the subgroup check (ecc/bn254/marshal.go:1116-1216, ecc/bls12-381/marshal.go:1160+), the same shape
+ * as the G1 pair: wire order X.A1 || X.A0 (|| Y.A1 || Y.A0), flags in the top byte of X.A1, compressed points take a square root
+ * of X^3 + b' in Fp2 (b' = bTwistCurveCoeff; "no root" decided by the norm, as E2.Legendre does) with the sign of
+ * E2.LexicographicallyLargest.  Output: the reference's in-memory G2Affine ({A0, A1} Montgomery limbs per coordinate, infinity =
+ * zeroes).  Groups: GMSM_BN254_G2, GMSM_BLS12381_G2, GMSM_BLS12377_G2, and GMSM_BW6761_G2 / GMSM_BW6633_G2 (curves over Fp, b' =
+ * 4 and 8: decoded by the G1 kernel); any other id is GMSM_EINVAL.  The device entry wants d_points 16-byte and d_first_error
+ * 8-byte aligned (GMSM_EINVAL otherwise). */
+int gmsm_g2_decode(gmsm_curve_t curve, const uint8_t* bytes, size_t n, int raw, int check_on_curve, uint64_t* out_points);
+int gmsm_g2_decode_device(gmsm_curve_t curve, const void* d_bytes, size_t n, int raw, int check_on_curve, void* d_points,
+                          void* d_first_error, void* stream);
+/* G1Affine / G2Affine Bytes (raw = 0: X with the smallest / largest / infinity flag, one coordinate's bytes per point) and
+ * RawBytes (raw = 1: X || Y; infinity is mUncompressedInfinity and zeroes, all zeroes on bn254), marshal.go:801-846 and
+ * :1051-1100, for the G1 and G2 groups of the seven pairing curves (secp256k1 and unknown ids: GMSM_EINVAL).  Points are the
+ * reference's in-memory affine points with reduced Montgomery limbs; n < 2^32.  The device entry is ordered on `stream` and
+ * allocates nothing; d_points must be 16-byte and d_bytes 4-byte aligned (GMSM_EINVAL otherwise). */
+int gmsm_points_encode(gmsm_curve_t curve, const uint64_t* points, size_t n, int raw, uint8_t* out);
+int gmsm_points_encode_device(gmsm_curve_t curve, const void* d_points, size_t n, int raw, void* d_bytes, void* stream);
 
 /* ---- next-row N3: Fr FFT behind gnark-crypto's fft.Domain (ecc/bn254/fr/fft/domain.go:24-110, fft.go:31-190,
  * bitreverse.go:17-42; the fr/fft packages of bls12-381, bls12-377, bls24-315, bls24-317, bw6-633 and bw6-761 are the same
