@@ -12,6 +12,7 @@ Layout:
                the one caller of the library's device Fr polynomial entry points
   iop.py       the Fr layer of a PLONK prover (ecc/<curve>/fr/iop): Polynomial and its forms, Evaluate of a traced expression, the
                accumulating ratios BuildRatioShuffledVectors / BuildRatioCopyConstraint and DivideByXMinusOne, all on the device
+  pairing.py   MillerLoop / FinalExponentiation / Pair / PairingCheck of bn254 and bls12-381 on the device
   mpcsetup.py  the point updates of a trusted-setup contribution (UpdateMonomialsG1/G2, ScaleG1/G2) and the linear combinations of
                SameRatioMany (LinearCombinationsG1/G2)
 """

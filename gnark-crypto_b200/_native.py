@@ -56,6 +56,13 @@ _SIGNATURES = [
     ("gmsm_g1_decode_device", i32, [i32, vp, sz, i32, i32, vp, vp, vp]),
     ("gmsm_g2_decode", i32, [i32, vp, sz, i32, i32, vp]),
     ("gmsm_g2_decode_device", i32, [i32, vp, sz, i32, i32, vp, vp, vp]),
+    ("gmsm_pairing_workspace_bytes", sz, [i32, sz]),
+    ("gmsm_pairing_miller_loop", i32, [i32, vp, vp, sz, vp]),
+    ("gmsm_pairing_miller_loop_device", i32, [i32, vp, vp, sz, vp, vp, vp]),
+    ("gmsm_pairing_final_exp", i32, [i32, vp, sz, vp]),
+    ("gmsm_pairing_final_exp_device", i32, [i32, vp, sz, vp, vp]),
+    ("gmsm_pair", i32, [i32, vp, vp, sz, vp]),
+    ("gmsm_pair_device", i32, [i32, vp, vp, sz, vp, vp, vp]),
     ("gmsm_points_encode", i32, [i32, vp, sz, i32, vp]),
     ("gmsm_points_encode_device", i32, [i32, vp, sz, i32, vp, vp]),
     ("gmsm_fft_fr_bytes", sz, [i32]),

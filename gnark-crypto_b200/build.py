@@ -20,7 +20,7 @@ FLAGS = [
     "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
-UNITS = ["gmsm.cu", "fft.cu", "decode.cu", "inst_bn254_g1.cu", "inst_bn254_g2.cu", "inst_bls12381_g1.cu", "inst_bls12381_g2.cu", "inst_bls12377_g1.cu", "inst_bls12377_g2.cu",
+UNITS = ["gmsm.cu", "fft.cu", "decode.cu", "pairing.cu", "inst_bn254_g1.cu", "inst_bn254_g2.cu", "inst_bls12381_g1.cu", "inst_bls12381_g2.cu", "inst_bls12377_g1.cu", "inst_bls12377_g2.cu",
          "inst_secp256k1_g1.cu", "inst_bw6761_g1.cu", "inst_bw6761_g2.cu",
          "inst_bls24315_g1.cu", "inst_bls24317_g1.cu", "inst_bw6633_g1.cu", "inst_bw6633_g2.cu"]
 

@@ -504,10 +504,18 @@ def _tonelli(a: int, p: int):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# batched openings at one point (kzg.go:246-420): the prover side; verification (pairings) is out of scope
+# batched openings at one point (kzg.go:246-420) and the verifiers
 # ----------------------------------------------------------------------------------------------------------------
 class ErrInvalidNbDigests(MultiExpError):
     """kzg.ErrInvalidNbDigests (kzg.go:23)"""
+
+
+class ErrZeroNbDigests(MultiExpError):
+    """kzg.ErrZeroNbDigests (kzg.go:24)"""
+
+
+class ErrVerifyOpeningProof(MultiExpError):
+    """kzg.ErrVerifyOpeningProof (kzg.go:26)"""
 
 
 @dataclass
@@ -853,3 +861,75 @@ def CommitLagrange(evals, pk: ProvingKey, domain) -> np.ndarray:
     domain.fft_device(d, True, DIF, False, st)          # natural in, bit-reversed out
     domain.bit_reverse_device(d, st)
     return _digest(pk._bases.MultiExpDevice(d, ev.shape[0], stream=st), pk.words)
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# verifiers (kzg.go:207-240, 385-500) on the GPU pairing (pairing.py).  The reference checks with PairingCheckFixedQ on the
+# precomputed lines of vk.G2; the general PairingCheck used here gives the same accept / reject for any input, because the two
+# Miller loops differ only by factors that the final exponentiation removes.
+# ----------------------------------------------------------------------------------------------------------------
+@dataclass
+class VerifyingKey:
+    """kzg.VerifyingKey (kzg.go:53-58): G2[0] the G2 generator, G2[1] = [alpha]G2, G1 the G1 generator (Go memory layout)"""
+
+    curve: str
+    G2: np.ndarray
+    G1: np.ndarray
+
+
+def _g1_msm(curve: str, points, scalars: list) -> np.ndarray:
+    """one affine G1 point: the MultiExp of `points` by the integers `scalars` (mod r)"""
+    from .multiexp import curve_package
+
+    cp = _params(curve)
+    pts = np.ascontiguousarray(np.stack([np.asarray(p, dtype=np.uint64).reshape(-1) for p in points]))
+    return curve_package(_curve(curve))[0]().MultiExp(pts, _fr_encode([k % cp.r for k in scalars], cp.r), MultiExpConfig()).limbs
+
+
+def _pairing_check(vk: VerifyingKey, a: np.ndarray, b: np.ndarray) -> bool:
+    """e(a, G2[0]) e(b, G2[1]) == 1"""
+    from . import pairing
+
+    g2 = np.ascontiguousarray(vk.G2, dtype=np.uint64).reshape(2, -1)
+    P = np.ascontiguousarray(np.stack([np.asarray(a, dtype=np.uint64).reshape(-1), np.asarray(b, dtype=np.uint64).reshape(-1)]))
+    return pairing.PairingCheck(_curve(vk.curve), P, g2)
+
+
+def Verify(commitment, proof: OpeningProof, point, vk: VerifyingKey) -> None:
+    """kzg.Verify (kzg.go:207-240): e([f(a) - a H(alpha) - f(alpha)]G1, G2) e([H(alpha)]G1, [alpha]G2) == 1, else
+    ErrVerifyOpeningProof.  The G1 combination is one MultiExp."""
+    r = _params(vk.curve).r
+    fa = _fr_decode(proof.ClaimedValue, r)[0]
+    a = _fr_decode(point, r)[0]
+    total = _g1_msm(vk.curve, [vk.G1, proof.H, commitment], [fa, -a, -1])
+    if not _pairing_check(vk, total, proof.H):
+        raise ErrVerifyOpeningProof("can't verify opening proof")
+
+
+def BatchVerifySinglePoint(digests, proof: BatchOpeningProof, point, hf, vk: VerifyingKey, *data_transcript: bytes) -> None:
+    """kzg.BatchVerifySinglePoint (kzg.go:385-400): FoldProof, then Verify of the folded proof"""
+    folded_proof, folded_digest = FoldProof(digests, proof, point, hf, vk.curve, *data_transcript)
+    Verify(folded_digest, folded_proof, point, vk)
+
+
+def BatchVerifyMultiPoints(digests, proofs, points, vk: VerifyingKey) -> None:
+    """kzg.BatchVerifyMultiPoints (kzg.go:405-500): with lambda_0 = 1 and random lambda_i (secrets), checks
+    e(sum lambda_i (C_i - [f_i(a_i)]G1 + [a_i]H_i), G2) e(-sum lambda_i H_i, [alpha]G2) == 1.  Each G1 side is one MultiExp."""
+    import secrets
+
+    if len(digests) != len(proofs) or len(digests) != len(points):
+        raise ErrInvalidNbDigests("number of digests is not the same as the number of polynomials")
+    if len(digests) == 0:
+        raise ErrZeroNbDigests("number of digests is zero")
+    if len(digests) == 1:
+        return Verify(digests[0], proofs[0], points[0], vk)
+    r = _params(vk.curve).r
+    lam = [1] + [secrets.randbelow(r) for _ in range(len(digests) - 1)]
+    evals = [_fr_decode(p.ClaimedValue, r)[0] for p in proofs]
+    a = [_fr_decode(x, r)[0] for x in points]
+    hs = [p.H for p in proofs]
+    folded_eval = sum(l * e for l, e in zip(lam, evals)) % r
+    folded_digests = _g1_msm(vk.curve, list(digests) + hs + [vk.G1], lam + [l * x for l, x in zip(lam, a)] + [-folded_eval])
+    folded_quotients = _g1_msm(vk.curve, hs, [-l for l in lam])
+    if not _pairing_check(vk, folded_digests, folded_quotients):
+        raise ErrVerifyOpeningProof("can't verify opening proof")

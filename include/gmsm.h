@@ -390,6 +390,24 @@ int gmsm_scale_powers(gmsm_curve_t curve, const uint64_t* points, size_t n, cons
 int gmsm_scale_powers_device(gmsm_curve_t curve, const void* d_points, size_t n, const uint64_t* c, const uint64_t* r, void* d_out,
                              void* stream);
 
+/* ---- pairings (bn254 and bls12-381) ----
+ * Pair, PairingCheck's pairing, MillerLoop and FinalExponentiation of ecc/bn254/pairing.go and ecc/bls12-381/pairing.go.  `curve` is
+ * the curve's G1 id (GMSM_BN254_G1 or GMSM_BLS12381_G1); any other id, n = 0 (the reference's "invalid inputs sizes") or a null
+ * pointer is GMSM_EINVAL before any device work.  P: n G1Affine, Q: n G2Affine (reference layout, infinity = zeroes; a pair with a
+ * point at infinity is skipped).  A GT element is E12{C0, C1} of E6{B0, B1, B2} of E2{A0, A1}: 12 Montgomery fp.Elements (48 u64
+ * for bn254, 72 for bls12-381).  MillerLoop's result is limb-identical to the reference's multi-pair loop; final_exp raises the
+ * product z[0] ... z[k-1] (k >= 1, the variadic form) to the reference's exponent.  The device entries take device buffers,
+ * 16-byte aligned (GMSM_EINVAL otherwise), are ordered on `stream` and allocate nothing: the Miller loop and Pair use d_work of
+ * gmsm_pairing_workspace_bytes(curve, n) bytes (the pairs run in chunks, so it stays bounded for any n < 2^32). */
+size_t gmsm_pairing_workspace_bytes(gmsm_curve_t curve, size_t n);
+int gmsm_pairing_miller_loop(gmsm_curve_t curve, const uint64_t* P, const uint64_t* Q, size_t n, uint64_t* out);
+int gmsm_pairing_miller_loop_device(gmsm_curve_t curve, const void* d_P, const void* d_Q, size_t n, void* d_out, void* d_work,
+                                    void* stream);
+int gmsm_pairing_final_exp(gmsm_curve_t curve, const uint64_t* z, size_t k, uint64_t* out);
+int gmsm_pairing_final_exp_device(gmsm_curve_t curve, const void* d_z, size_t k, void* d_out, void* stream);
+int gmsm_pair(gmsm_curve_t curve, const uint64_t* P, const uint64_t* Q, size_t n, uint64_t* out);
+int gmsm_pair_device(gmsm_curve_t curve, const void* d_P, const void* d_Q, size_t n, void* d_out, void* d_work, void* stream);
+
 /* ---- 5. test hooks: element-wise device functions, used by tests/ to check the sm_90a field and
  * point arithmetic against the oracle.  a, b, out are HOST arrays of n elements each. ---- */
 enum {

@@ -133,6 +133,46 @@ std::vector<typename G1::Affine> to_lagrange_g1(const std::vector<typename G1::A
     return to_lagrange_g1<G1>(coeffs, device);                                                                       \
   }
 
+// pairing.go MillerLoop / FinalExponentiation / Pair / PairingCheck for bn254 and bls12-381 (gmsm_pair*): GT = E12 as 12
+// Montgomery fp.Elements.  Wrapped below in the two curve namespaces.
+template <class G1, class G2, int L>
+struct Pairing {
+  using GT = std::array<uint64_t, 12 * L>;
+  static void sizes(size_t np, size_t nq) {
+    if (np == 0 || np != nq) throw Error("invalid inputs sizes");
+  }
+  static GT MillerLoop(const std::vector<typename G1::Affine>& P, const std::vector<typename G2::Affine>& Q) {
+    sizes(P.size(), Q.size());
+    GT out{};
+    if (gmsm_pairing_miller_loop(G1::curve, P[0].X.data(), Q[0].X.data(), P.size(), out.data()) != GMSM_OK) throw Error(gmsm_last_error());
+    return out;
+  }
+  static GT FinalExponentiation(const GT& z, const std::vector<GT>& zs = {}) {
+    std::vector<GT> all{z};
+    all.insert(all.end(), zs.begin(), zs.end());
+    GT out{};
+    if (gmsm_pairing_final_exp(G1::curve, all[0].data(), all.size(), out.data()) != GMSM_OK) throw Error(gmsm_last_error());
+    return out;
+  }
+  static GT Pair(const std::vector<typename G1::Affine>& P, const std::vector<typename G2::Affine>& Q) {
+    sizes(P.size(), Q.size());
+    GT out{};
+    if (gmsm_pair(G1::curve, P[0].X.data(), Q[0].X.data(), P.size(), out.data()) != GMSM_OK) throw Error(gmsm_last_error());
+    return out;
+  }
+  // Pair(P, Q) == 1; the one of GT is the Miller loop of a pair at infinity, which the library returns as 1
+  static bool PairingCheck(const std::vector<typename G1::Affine>& P, const std::vector<typename G2::Affine>& Q) {
+    const GT f = Pair(P, Q);
+    return f == MillerLoop({typename G1::Affine{}}, {typename G2::Affine{}});
+  }
+};
+#define GMSM_HOST_PAIRING(L)                                                                                                        \
+  using GT = Pairing<G1, G2, L>::GT;                                                                                                \
+  inline GT MillerLoop(const std::vector<G1Affine>& P, const std::vector<G2Affine>& Q) { return Pairing<G1, G2, L>::MillerLoop(P, Q); } \
+  inline GT FinalExponentiation(const GT& z, const std::vector<GT>& zs = {}) { return Pairing<G1, G2, L>::FinalExponentiation(z, zs); } \
+  inline GT Pair(const std::vector<G1Affine>& P, const std::vector<G2Affine>& Q) { return Pairing<G1, G2, L>::Pair(P, Q); }            \
+  inline bool PairingCheck(const std::vector<G1Affine>& P, const std::vector<G2Affine>& Q) { return Pairing<G1, G2, L>::PairingCheck(P, Q); }
+
 namespace bn254 {
 using G1 = Group<GMSM_BN254_G1, 4, 1>;
 using G2 = Group<GMSM_BN254_G2, 4, 2>;
@@ -141,6 +181,7 @@ using G1Jac = G1::Jac;
 using G2Affine = G2::Affine;
 using G2Jac = G2::Jac;
 GMSM_HOST_TO_LAGRANGE
+GMSM_HOST_PAIRING(4)
 }  // namespace bn254
 namespace bls12381 {
 using G1 = Group<GMSM_BLS12381_G1, 6, 1>;
@@ -150,6 +191,7 @@ using G1Jac = G1::Jac;
 using G2Affine = G2::Affine;
 using G2Jac = G2::Jac;
 GMSM_HOST_TO_LAGRANGE
+GMSM_HOST_PAIRING(6)
 }  // namespace bls12381
 namespace bls12377 {   // ecc/bls12-377
 using G1 = Group<GMSM_BLS12377_G1, 6, 1>;
