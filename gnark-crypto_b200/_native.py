@@ -50,6 +50,7 @@ _SIGNATURES = [
     ("gmsm_ctx_finalize_device", i32, [vp, vp, i32, vp, vp]),
     ("gmsm_ctx_set_profiling", None, [vp, i32]),
     ("gmsm_ctx_last_stage_ms", i32, [vp, ctypes.POINTER(ctypes.c_float)]),
+    ("gmsm_ctx_last_timeline_ms", i32, [vp, ctypes.POINTER(ctypes.c_float), i32, ctypes.POINTER(ctypes.c_int)]),
     ("gmsm_generate_multiples_device", i32, [i32, vp, u64, sz, vp, vp]),
     ("gmsm_batch_scalar_mul", i32, [i32, vp, vp, sz, vp]),
     ("gmsm_g1_decode", i32, [i32, vp, sz, i32, i32, vp]),

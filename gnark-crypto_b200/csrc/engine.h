@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <mutex>
 #include <string>
+#include <vector>
 
 #include "../../include/gmsm.h"
 #include "groups.cuh"
@@ -103,9 +104,14 @@ struct gmsm_ctx {
   size_t max_chunks = 0;
   size_t ws_bytes = 0;
   int last_launches = 0;
-  bool profiling = false;
+  int profiling = 0;                   // 1: stage events (ev); 2: also the scatter / accumulate timeline (tl_ev)
   cudaEvent_t ev[9] = {};
-  int split_w = 2;                     // windows scattered before the accumulate starts (GMSM_SPLIT_W)
+  // timeline of the last profiled call at level 2: events before and after every scatter pass (2 per pass, on the stream it
+  // ran on), then before / after accumulate part 1 (or the only part) and part 2 -- part 2's "before" is recorded after the
+  // wait for the auxiliary stream.  Created on first use.
+  std::vector<cudaEvent_t> tl_ev;
+  int tl_npass = 0, tl_split = 0, tl_parts = 0;
+  int split_w = 4;                     // windows scattered before the accumulate starts (GMSM_SPLIT_W)
   int split_tab = 1;                   // the same for the bucket-range passes of the window-table mode
   cudaStream_t aux = nullptr;          // auxiliary stream: scatter of the later windows under the accumulate
   cudaEvent_t ev_split[2] = {};

@@ -30,6 +30,7 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
   if (n == 0) {
     if (!rmw) CK(cudaMemsetAsync(buckets, 0, (size_t)p.nb_total * sizeof(X), st));
     for (int i = 1; i <= 5; i++) mark(i);
+    c->tl_npass = c->tl_parts = 0;
     c->last_launches = 0;
     return GMSM_OK;
   }
@@ -55,22 +56,27 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
   }
   mark(1);
   // K1b: scan
-  auto scan_u32 = [&](const uint32_t* in, uint32_t* out) -> int {
+  // ends: the counters `in` become bucket end pointers as well (the histogram, for the scatter)
+  auto scan_u32 = [&](uint32_t* in, uint32_t* out, bool ends) -> int {
     unsigned nb_blocks = nblk(nbp, SCAN_TILE);
     k_scan_block_sums<<<nb_blocks, SCAN_THREADS, 0, st>>>(in, (uint32_t)nbp, c->block_sums);
     k_scan_top<<<1, 1024, 0, st>>>(c->block_sums, nb_blocks, c->block_sums + nb_blocks);
-    k_scan_final<<<nb_blocks, SCAN_THREADS, 0, st>>>(in, (uint32_t)nbp, c->block_sums, out);
+    if (ends)
+      k_scan_final_ends<<<nb_blocks, SCAN_THREADS, 0, st>>>(in, (uint32_t)nbp, c->block_sums, out);
+    else
+      k_scan_final<<<nb_blocks, SCAN_THREADS, 0, st>>>(in, (uint32_t)nbp, c->block_sums, out);
     launches += 3;
     LAUNCH_CHECK();
     return GMSM_OK;
   };
-  if (int rc = scan_u32(c->hist, c->offsets)) return rc;
+  if (int rc = scan_u32(c->hist, c->offsets, true)) return rc;
   mark(2);
   // K1c: scatter, one launch per window (L2-resident write set).  In the extended-Jacobian mode only the
   // first SPLIT_W windows are scattered on the call's stream; the rest go to the context's auxiliary stream
   // and run underneath the first part of the accumulate kernel (multiplier-bound, L2 idle) -- see K2.
   // (faster for the G1 groups; slower for G2, whose 255-register accumulate blocks leave no room for co-resident
-  // scatter blocks -> G1 groups only)
+  // scatter blocks -> G1 groups only.)  SPLIT_W = 4 by default: at bn254 G1 n = 2^24 (15 windows) part 1 then lasts long
+  // enough for the other 11 windows to be scattered underneath it, and part 2 hardly waits (DESIGN.md section 5).
   // Window-table mode: one pass per bucket range instead of one per window (k_scatter_shared); the ranges play
   // the role of the windows for the overlap with the accumulate.
   // (timed at bn254 G1 n = 2^24, c = 22: every pass streams all n*W digits, so few passes win even though a pass's
@@ -82,19 +88,46 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
   }
   const uint32_t range_sz = c->shared ? (p.nb_total + (uint32_t)NPASS - 1) / (uint32_t)NPASS : p.nb;
   const int SPLIT_W = (!c->affine && sizeof(F) <= 48 && p.nwin >= 6 && n >= (1u << 16)) ? std::min(c->shared ? c->split_tab : c->split_w, NPASS) : NPASS;
-  const unsigned scatter_blocks = std::min<unsigned>(nblk(n, 256 * 4), GMSM_NUM_SMS * (c->shared ? 2u : 8u));
+  // The counters in hist are bucket end pointers (k_scan_final_ends): the scatters take their positions from them and get no
+  // offsets.  On the auxiliary stream the slim form (k_scatter_window_aux, one block per SM) so that it shares the SMs with
+  // the accumulate; that stream has the highest priority (gmsm.cu, ctx_alloc).
+  const unsigned scatter_blocks = std::min<unsigned>(nblk(n, 256 * SCATTER_U), GMSM_NUM_SMS * (unsigned)SCATTER_BLOCKS_PER_SM);
+  const unsigned scatter_blocks_aux = std::min<unsigned>(nblk(n, 256 * SCATTER_AUX_U), GMSM_NUM_SMS * (unsigned)SCATTER_AUX_BLOCKS_PER_SM);
+  const unsigned shared_blocks = std::min<unsigned>(nblk(n, 256 * 4), GMSM_NUM_SMS * 2u);
+  // profiling level 2: events around every scatter pass and the accumulate parts (gmsm_ctx_last_timeline_ms)
+  const bool timeline = c->profiling >= 2;
+  if (timeline) {
+    while (c->tl_ev.size() < (size_t)NPASS * 2 + 4) {
+      cudaEvent_t e;
+      CK(cudaEventCreate(&e));
+      c->tl_ev.push_back(e);
+    }
+    c->tl_npass = NPASS;
+    c->tl_split = std::min(SPLIT_W, NPASS);
+    c->tl_parts = 0;
+  }
+  auto tl = [&](size_t i, cudaStream_t s) { if (timeline) cudaEventRecord(c->tl_ev[i], s); };
   auto scatter = [&](int r, cudaStream_t s) {   // pass r: bucket range r (window-table mode) or window r
+    tl(2 * (size_t)r, s);
     if (c->shared) {
       const uint32_t blo = std::min<uint64_t>((uint64_t)r * range_sz, p.nb_total);
       const uint32_t bhi = std::min<uint64_t>((uint64_t)(r + 1) * range_sz, p.nb_total);
-      if (blo >= bhi) return;
-      k_scatter_shared<<<dim3(scatter_blocks, (unsigned)p.nwin), 256, 0, s>>>(c->digits, c->ranks, n32, c->tab_stride, c->hist,
-                                                                               c->offsets, c->entries, blo, bhi, c->hist + nbp + 4);
+      if (blo < bhi) {
+        k_scatter_shared<<<dim3(shared_blocks, (unsigned)p.nwin), 256, 0, s>>>(c->digits, c->ranks, n32, c->tab_stride, c->hist,
+                                                                              nullptr, c->entries, blo, bhi, c->hist + nbp + 4);
+        launches++;
+      }
     } else {
-      k_scatter_window<<<scatter_blocks, 256, 0, s>>>(c->digits + (size_t)r * n, c->ranks + (size_t)r * n, n32, c->hist + (size_t)r * p.nb,
-                                                      c->offsets + (size_t)r * p.nb, c->entries, c->hist + nbp + 4);
+      const uint32_t* dw = c->digits + (size_t)r * n;
+      const uint32_t* rw = c->ranks + (size_t)r * n;
+      uint32_t* ends = c->hist + (size_t)r * p.nb;
+      if (s == st)
+        k_scatter_window<<<scatter_blocks, 256, 0, s>>>(dw, rw, n32, ends, nullptr, c->entries, c->hist + nbp + 4);
+      else
+        k_scatter_window_aux<<<scatter_blocks_aux, 256, 0, s>>>(dw, rw, n32, ends, nullptr, c->entries, c->hist + nbp + 4);
+      launches++;
     }
-    launches++;
+    tl(2 * (size_t)r + 1, s);
   };
   if (SPLIT_W < NPASS) {
     CK(cudaEventRecord(c->ev_split[0], st));           // scan done: offsets, digits, hist are ready
@@ -129,7 +162,7 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
       uint32_t* off_next = c->aff_off[l & 1];
       k_aff_level_counts<<<std::min<unsigned>(nblk(nbp, 256), GMSM_NUM_SMS * 8u), 256, 0, st>>>(c->offsets, nbt, l + 1, c->aff_counts);
       launches++;
-      if (int rc = scan_u32(c->aff_counts, off_next)) return rc;
+      if (int rc = scan_u32(c->aff_counts, off_next, false)) return rc;
       // sum_b ceil(len_b/2) <= (m + #nonempty)/2 and #nonempty <= min(nb, m): non-increasing bound
       const size_t m_next = std::min(m_up, (m_up + std::min<size_t>(nbt, m_up)) / 2 + 1);
       uint32_t B = 8;
@@ -174,18 +207,26 @@ static int run_accumulate(gmsm_ctx* c, const void* d_points, const void* d_scala
     CK(cudaMemsetAsync(buckets, 0, (size_t)p.nb_total * sizeof(X), st));
     {
       X* carr = reinterpret_cast<X*>(c->carries[0]);
+      const size_t t0 = 2 * (size_t)NPASS;   // timeline slots of the accumulate parts
+      tl(t0, st);
       if (SPLIT_W < NPASS) {
         const uint32_t split_bucket = (uint32_t)std::min<uint64_t>((uint64_t)SPLIT_W * range_sz, p.nb_total);
         k_accumulate<G><<<nblk(nchunks, 128), 128, 0, st>>>(points, c->entries, c->offsets, p.nb_total, K, (uint32_t)nchunks,
                                                             buckets, carr, c->carry_ids[0], 1, split_bucket);
+        tl(t0 + 1, st);
         CK(cudaStreamWaitEvent(st, c->ev_split[1], 0));   // the remaining windows are scattered
+        tl(t0 + 2, st);
         k_accumulate<G><<<nblk(nchunks, 128), 128, 0, st>>>(points, c->entries, c->offsets, p.nb_total, K, (uint32_t)nchunks,
                                                             buckets, carr, c->carry_ids[0], 2, split_bucket);
+        tl(t0 + 3, st);
         launches += 2;
+        if (timeline) c->tl_parts = 2;
       } else {
         k_accumulate<G><<<nblk(nchunks, 128), 128, 0, st>>>(points, c->entries, c->offsets, p.nb_total, K, (uint32_t)nchunks,
                                                             buckets, carr, c->carry_ids[0], 0, 0);
+        tl(t0 + 1, st);
         launches++;
+        if (timeline) c->tl_parts = 1;
       }
       LAUNCH_CHECK();
     }

@@ -239,7 +239,14 @@ static int ctx_alloc(gmsm_ctx* c) {
   CK(dmalloc(&c->fin_scratch, (size_t)p.nwin * xyzz, &acc));
   c->ws_bytes = acc;
   for (int i = 0; i < 9; i++) CK(cudaEventCreate(&c->ev[i]));
-  CK(cudaStreamCreateWithFlags(&c->aux, cudaStreamNonBlocking));
+  // the auxiliary stream carries only the scatter that runs underneath the accumulate (engine_impl.cuh, K1c).  At the highest
+  // priority the block scheduler places its blocks whenever an accumulate block leaves an SM; at the default priority the
+  // pending accumulate blocks took those slots first and most of the scatter waited for the end of part 1.
+  {
+    int lo = 0, hi = 0;
+    CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+    CK(cudaStreamCreateWithPriority(&c->aux, cudaStreamNonBlocking, hi));
+  }
   for (int i = 0; i < 2; i++) CK(cudaEventCreateWithFlags(&c->ev_split[i], cudaEventDisableTiming));
   CK(cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming));
   return GMSM_OK;
@@ -281,6 +288,7 @@ static void ctx_free(gmsm_ctx* c) {
   cudaFree(c->aff_maxlen);
   if (c->aff_maxlen_host) cudaFreeHost(c->aff_maxlen_host);
   for (int i = 0; i < 9; i++) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
+  for (cudaEvent_t e : c->tl_ev) cudaEventDestroy(e);
   for (int i = 0; i < 2; i++) if (c->ev_split[i]) cudaEventDestroy(c->ev_split[i]);
   if (c->aux) cudaStreamDestroy(c->aux);
   if (c->ev_done) cudaEventDestroy(c->ev_done);
@@ -358,7 +366,7 @@ extern "C" int gmsm_ctx_window_bits(const gmsm_ctx_t* ctx) { return ctx ? ctx->p
 extern "C" int gmsm_ctx_num_windows(const gmsm_ctx_t* ctx) { return ctx ? ctx->plan.nwin : 0; }
 extern "C" size_t gmsm_ctx_workspace_bytes(const gmsm_ctx_t* ctx) { return ctx ? ctx->ws_bytes : 0; }
 extern "C" int gmsm_ctx_last_launches(const gmsm_ctx_t* ctx) { return ctx ? ctx->last_launches : 0; }
-extern "C" void gmsm_ctx_set_profiling(gmsm_ctx_t* ctx, int on) { if (ctx) ctx->profiling = on != 0; }
+extern "C" void gmsm_ctx_set_profiling(gmsm_ctx_t* ctx, int on) { if (ctx) ctx->profiling = on >= 2 ? 2 : (on != 0); }
 extern "C" int gmsm_ctx_last_stage_ms(gmsm_ctx_t* ctx, float out_ms[8]) {
   if (!ctx || !ctx->have_stage) return set_err(GMSM_EINVAL, "no profiled call recorded");
   cudaSetDevice(ctx->device);
@@ -369,6 +377,26 @@ extern "C" int gmsm_ctx_last_stage_ms(gmsm_ctx_t* ctx, float out_ms[8]) {
   }
   CK(cudaEventElapsedTime(&tot, ctx->ev[0], ctx->ev[7]));
   out_ms[7] = tot;
+  return GMSM_OK;
+}
+
+extern "C" int gmsm_ctx_last_timeline_ms(gmsm_ctx_t* ctx, float* out_ms, int cap, int* count) {
+  if (!ctx || !count) return set_err(GMSM_EINVAL, "null argument");
+  if (!ctx->have_stage || ctx->profiling < 2 || ctx->tl_parts == 0) return set_err(GMSM_EINVAL, "no timeline recorded (profiling level 2)");
+  const int need = 3 + 2 * ctx->tl_npass + 4;
+  *count = need;
+  if (!out_ms || cap < need) return set_err(GMSM_EINVAL, "timeline needs %d values, got room for %d", need, cap);
+  cudaSetDevice(ctx->device);
+  out_ms[0] = (float)ctx->tl_npass;
+  out_ms[1] = (float)ctx->tl_split;
+  out_ms[2] = (float)ctx->tl_parts;
+  const int nev = 2 * ctx->tl_npass + 2 * ctx->tl_parts;
+  for (int i = 0; i < 2 * ctx->tl_npass + 4; i++) {
+    out_ms[3 + i] = -1.0f;
+    if (i >= nev) continue;
+    CK(cudaEventSynchronize(ctx->tl_ev[i]));
+    CK(cudaEventElapsedTime(&out_ms[3 + i], ctx->ev[0], ctx->tl_ev[i]));
+  }
   return GMSM_OK;
 }
 

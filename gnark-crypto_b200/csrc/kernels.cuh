@@ -219,21 +219,31 @@ __global__ void k_digits_hist(const typename G::Fr* __restrict__ scalars, uint32
   }
 }
 
-// K1c: scatter of ONE window: entries[offsets[b] + position] = (i << 1) | sign, the position taken from ranks[] (rank mode) or
-// with a returning atomicSub on the bucket's counter (plain mode: filled from the back, the histogram counts down to zero).
+// K1c: scatter of ONE window: entries[position] = (i << 1) | sign.  The engine launches it after k_scan_final_ends, which
+// turned the window's counters hist_w[] into bucket END pointers (offsets_w == nullptr): in plain mode the returning
+// atomicSub on the counter IS the position (buckets fill from the back, each counter ends at its bucket's offset), so an
+// entry costs one atomic and one store; in rank mode the position is end - 1 - rank.  With offsets_w the counters hold
+// counts and the positions are offsets_w[b] + (count - 1, count - 2, ...) or offsets_w[b] + rank (the counters then count
+// down to zero): the form the CPU emulation of the pipeline drives (tests/emu/emu_engine.cpp, with a host scan).
 // Launched window by window so that the randomly written slice of `entries` (<= 4n bytes) and the window's counters stay
 // L2-resident and reach HBM once, as full lines, instead of one read-modify-write per 4-byte store.  H100 has 50 MB of L2, so
 // the slice fits up to n ~ 2^23; at n = 2^24 (64 MiB) it spills partly, yet the exposed scatter still costs the same per point
 // as at n = 2^20 (DESIGN.md section 3).  Well beyond that (2^26) the cost per point about doubles; a window split into bucket
 // ranges that fit L2 (what k_scatter_shared does for the window-table mode) would address it and is not done here.
-static __global__ void k_scatter_window(const uint32_t* __restrict__ digits_w, const uint32_t* __restrict__ ranks_w, uint32_t n,
-                                        uint32_t* __restrict__ hist_w, const uint32_t* __restrict__ offsets_w, uint32_t* __restrict__ entries,
-                                        const uint32_t* __restrict__ skew_flag) {
-  constexpr int U = 4;   // independent elements per thread and iteration (the plain mode is bound by the round trip of its atomics)
+GMSM_D uint32_t scatter_position(uint32_t* __restrict__ counters, const uint32_t* __restrict__ offsets, uint32_t b, bool rank_mode,
+                                 uint32_t rk) {
+  if (offsets == nullptr) return rank_mode ? counters[b] - 1u - rk : atomicSub(&counters[b], 1u) - 1u;
+  return offsets[b] + (rank_mode ? rk : atomicSub(&counters[b], 1u) - 1u);
+}
+// U independent entries per thread and iteration: the atomics of all U are in flight together
+template <int U>
+GMSM_D void scatter_window(const uint32_t* __restrict__ digits_w, const uint32_t* __restrict__ ranks_w, uint32_t n,
+                           uint32_t* __restrict__ hist_w, const uint32_t* __restrict__ offsets_w, uint32_t* __restrict__ entries,
+                           const uint32_t* __restrict__ skew_flag) {
   const bool rank_mode = skew_flag[0] != 0;
   const uint32_t tile = blockDim.x * U;
   for (uint64_t base = (uint64_t)blockIdx.x * tile; base < n; base += (uint64_t)gridDim.x * tile) {
-    uint32_t code[U], rk[U], off[U];
+    uint32_t code[U], rk[U], pos[U];
 #pragma unroll
     for (int u = 0; u < U; u++) {
       const uint64_t i = base + (uint64_t)u * blockDim.x + threadIdx.x;
@@ -241,28 +251,40 @@ static __global__ void k_scatter_window(const uint32_t* __restrict__ digits_w, c
       rk[u] = (rank_mode && code[u]) ? __ldg(ranks_w + i) : 0u;
     }
 #pragma unroll
-    for (int u = 0; u < U; u++) {
-      if (code[u]) {
-        const uint32_t b = code_bucket(code[u]);
-        if (!rank_mode) rk[u] = atomicSub(&hist_w[b], 1u) - 1u;
-        off[u] = offsets_w[b];
-      }
-    }
+    for (int u = 0; u < U; u++)
+      if (code[u]) pos[u] = scatter_position(hist_w, offsets_w, code_bucket(code[u]), rank_mode, rk[u]);
 #pragma unroll
     for (int u = 0; u < U; u++) {
       if (code[u]) {
         const uint32_t i = (uint32_t)(base + (uint64_t)u * blockDim.x + threadIdx.x);
-        entries[off[u] + rk[u]] = (i << 1) | (code[u] & 1u);
+        entries[pos[u]] = (i << 1) | (code[u] & 1u);
       }
     }
   }
 }
+// on the call's stream, where the scatter has the machine to itself: SCATTER_BLOCKS_PER_SM blocks of 256 threads per SM
+static constexpr int SCATTER_U = 4, SCATTER_BLOCKS_PER_SM = 8;
+static __global__ void k_scatter_window(const uint32_t* __restrict__ digits_w, const uint32_t* __restrict__ ranks_w, uint32_t n,
+                                        uint32_t* __restrict__ hist_w, const uint32_t* __restrict__ offsets_w, uint32_t* __restrict__ entries,
+                                        const uint32_t* __restrict__ skew_flag) {
+  scatter_window<SCATTER_U>(digits_w, ranks_w, n, hist_w, offsets_w, entries, skew_flag);
+}
+// on the auxiliary stream, underneath the accumulate: ONE block of 256 threads per SM with twice the entries per thread.  A window
+// takes about as long as with the full grid (the scatter is bound by the L2's atomics, not by the threads in flight), and the
+// block (44 registers per thread) fits beside three k_accumulate blocks of the 8-limb groups, which fill the register file at four.
+static constexpr int SCATTER_AUX_U = 8, SCATTER_AUX_BLOCKS_PER_SM = 1;
+static __global__ void k_scatter_window_aux(const uint32_t* __restrict__ digits_w, const uint32_t* __restrict__ ranks_w, uint32_t n,
+                                            uint32_t* __restrict__ hist_w, const uint32_t* __restrict__ offsets_w, uint32_t* __restrict__ entries,
+                                            const uint32_t* __restrict__ skew_flag) {
+  scatter_window<SCATTER_AUX_U>(digits_w, ranks_w, n, hist_w, offsets_w, entries, skew_flag);
+}
 
 // K1c (window-table mode, see k_table_level): all W windows feed ONE bucket set -- the entry of (scalar i,
 // window j) is the table point j*row_stride + i = 2^(c*j) * P_i, and hist / offsets / ranks are indexed by the bucket
-// alone.  The L2-residency argument of k_scatter_window is kept by passing over the digits once per BUCKET RANGE
-// [blo, bhi): a range owns a contiguous slice of `entries` (~4n bytes for uniform digits), every pass streams
-// all n*W digits (coalesced) and scatters only the ones of its range.  blockIdx.y = window.
+// alone (hist holds end pointers when offsets is null, as in k_scatter_window).  The L2-residency argument of
+// k_scatter_window is kept by passing over the digits once per BUCKET RANGE [blo, bhi): a range owns a contiguous slice of
+// `entries` (~4n bytes for uniform digits), every pass streams all n*W digits (coalesced) and scatters only the ones of its
+// range.  blockIdx.y = window.
 static __global__ void k_scatter_shared(const uint32_t* __restrict__ digits, const uint32_t* __restrict__ ranks, uint32_t n, uint32_t row_stride,
                                         uint32_t* __restrict__ hist, const uint32_t* __restrict__ offsets, uint32_t* __restrict__ entries,
                                         uint32_t blo, uint32_t bhi, const uint32_t* __restrict__ skew_flag) {
@@ -274,7 +296,7 @@ static __global__ void k_scatter_shared(const uint32_t* __restrict__ digits, con
   const uint32_t* ranks_w = ranks + (size_t)j * n;
   const uint32_t idx0 = j * row_stride;      // (W * row_stride) < 2^31 is checked by the host
   for (uint64_t base = (uint64_t)blockIdx.x * tile; base < n; base += (uint64_t)gridDim.x * tile) {
-    uint32_t code[U], rk[U], off[U];
+    uint32_t code[U], rk[U], pos[U];
 #pragma unroll
     for (int u = 0; u < U; u++) {
       const uint64_t i = base + (uint64_t)u * blockDim.x + threadIdx.x;
@@ -286,18 +308,13 @@ static __global__ void k_scatter_shared(const uint32_t* __restrict__ digits, con
       rk[u] = (rank_mode && code[u]) ? __ldg(ranks_w + i) : 0u;
     }
 #pragma unroll
-    for (int u = 0; u < U; u++) {
-      if (code[u]) {
-        const uint32_t b = code_bucket(code[u]);
-        if (!rank_mode) rk[u] = atomicSub(&hist[b], 1u) - 1u;
-        off[u] = offsets[b];
-      }
-    }
+    for (int u = 0; u < U; u++)
+      if (code[u]) pos[u] = scatter_position(hist, offsets, code_bucket(code[u]), rank_mode, rk[u]);
 #pragma unroll
     for (int u = 0; u < U; u++) {
       if (code[u]) {
         const uint32_t i = (uint32_t)(base + (uint64_t)u * blockDim.x + threadIdx.x);
-        entries[off[u] + rk[u]] = ((idx0 + i) << 1) | (code[u] & 1u);
+        entries[pos[u]] = ((idx0 + i) << 1) | (code[u] & 1u);
       }
     }
   }
@@ -373,8 +390,9 @@ static __global__ void k_scan_top(uint32_t* __restrict__ block_sums, uint32_t nb
   if (threadIdx.x == 0) *grand = running;
 }
 
-static __global__ void k_scan_final(const uint32_t* __restrict__ in, uint32_t n, const uint32_t* __restrict__ block_sums,
-                             uint32_t* __restrict__ out) {
+template <bool ENDS>
+GMSM_D void scan_final_tile(const uint32_t* in, uint32_t n, const uint32_t* __restrict__ block_sums, uint32_t* __restrict__ out,
+                            uint32_t* ends) {
   __shared__ uint32_t smem[33];
   uint32_t base = blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
   uint32_t v[SCAN_ITEMS];
@@ -388,9 +406,22 @@ static __global__ void k_scan_final(const uint32_t* __restrict__ in, uint32_t n,
   uint32_t ex = block_excl_scan(s, smem, &tot) + block_sums[blockIdx.x];
 #pragma unroll
   for (int k = 0; k < SCAN_ITEMS; k++) {
-    if (base + k < n) out[base + k] = ex;
+    if (base + k < n) {
+      out[base + k] = ex;
+      if constexpr (ENDS) ends[base + k] = ex + v[k];
+    }
     ex += v[k];
   }
+}
+static __global__ void k_scan_final(const uint32_t* __restrict__ in, uint32_t n, const uint32_t* __restrict__ block_sums,
+                             uint32_t* __restrict__ out) {
+  scan_final_tile<false>(in, n, block_sums, out, nullptr);
+}
+// the same over the bucket histogram, which it also turns in place into bucket END pointers (offset + count): the scatter's
+// returning atomic on a counter then yields the entry's position directly (k_scatter_window)
+static __global__ void k_scan_final_ends(uint32_t* counts, uint32_t n, const uint32_t* __restrict__ block_sums,
+                                         uint32_t* __restrict__ out) {
+  scan_final_tile<true>(counts, n, block_sums, out, counts);
 }
 
 // first index in offsets[0..len) with offsets[idx] > key  (offsets non-decreasing)

@@ -284,14 +284,29 @@ class Engine:
         _check(rc)
         return out
 
-    def set_profiling(self, on: bool):
-        _native.lib().gmsm_ctx_set_profiling(self._h, 1 if on else 0)
+    def set_profiling(self, on):
+        """True / 1: stage timings (last_stage_ms); 2: also the scatter / accumulate timeline (last_timeline_ms)"""
+        _native.lib().gmsm_ctx_set_profiling(self._h, int(on))
 
     def last_stage_ms(self):
         buf = (ctypes.c_float * 8)()
         rc = _native.lib().gmsm_ctx_last_stage_ms(self._h, buf)
         _check(rc)
         return list(buf)
+
+    def last_timeline_ms(self):
+        """the last call's timeline (gmsm_ctx_last_timeline_ms) as a dict: passes = [(stream, start, end)] in pass order,
+        stream "main" or "aux"; parts = [(start, end)] of the accumulate parts; ms from the start of the call"""
+        L = _native.lib()
+        cnt = ctypes.c_int(0)
+        buf = (ctypes.c_float * 512)()
+        _check(L.gmsm_ctx_last_timeline_ms(self._h, buf, len(buf), ctypes.byref(cnt)))
+        v = list(buf)[: cnt.value]
+        npass, split, nparts = int(v[0]), int(v[1]), int(v[2])
+        ev = v[3:]
+        passes = [("main" if r < split else "aux", ev[2 * r], ev[2 * r + 1]) for r in range(npass)]
+        parts = [(ev[2 * npass + 2 * k], ev[2 * npass + 2 * k + 1]) for k in range(nparts)]
+        return {"passes": passes, "split": split, "parts": parts}
 
     @property
     def last_launches(self):

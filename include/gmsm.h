@@ -170,6 +170,13 @@ int gmsm_ctx_msm_tables_device(gmsm_ctx_t* ctx, const void* d_table, size_t row_
  * carries, bucket-reduce, finalize, total] */
 void gmsm_ctx_set_profiling(gmsm_ctx_t* ctx, int on);
 int gmsm_ctx_last_stage_ms(gmsm_ctx_t* ctx, float out_ms[8]);
+/* with gmsm_ctx_set_profiling(ctx, 2), the last call's scatter / accumulate timeline (CUDA events on the call's stream and on
+ * the context's auxiliary stream), in milliseconds from the start of the call: out_ms[0] = P scatter passes, [1] = passes
+ * scattered on the call's stream ahead of the accumulate (the others ran on the auxiliary stream), [2] = accumulate parts (1
+ * or 2); then start, end of pass 0 .. P-1; then start, end of accumulate part 1 (or of the only part) and of part 2 (-1 when
+ * there is none), part 2's start being the end of its wait for the auxiliary stream.  *count = 3 + 2P + 4 values; GMSM_EINVAL
+ * when cap is smaller or no timeline was recorded (the batch-affine mode records none). */
+int gmsm_ctx_last_timeline_ms(gmsm_ctx_t* ctx, float* out_ms, int cap, int* count);
 
 /* ---- 4. base generation (fixed-base helper, SURVEY.md N1/K6): out[i] = [start + i] * base, affine,
  * device pointers; used to build on-curve benchmark inputs without the Go toolchain ---- */
