@@ -101,6 +101,7 @@ _SIGNATURES = [
     ("gmsm_scale_powers", i32, [i32, vp, sz, vp, vp, i32, vp]),
     ("gmsm_scale_powers_device", i32, [i32, vp, sz, vp, vp, vp, vp]),
     ("gmsm_test_op", i32, [i32, i32, vp, vp, vp, sz]),
+    ("gmsm_test_tower_op", i32, [i32, i32, vp, vp, vp, sz]),
     ("gmsm_test_digits", i32, [i32, i32, vp, sz, vp]),
 ]
 SYMBOLS = [name for name, _, _ in _SIGNATURES]

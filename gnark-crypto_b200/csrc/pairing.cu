@@ -8,6 +8,7 @@
 #include "engine.h"
 
 #include "pairing_kernels.cuh"
+#include "tower_testops.cuh"
 
 using namespace gmsm;
 
@@ -149,4 +150,29 @@ extern "C" int gmsm_pair(gmsm_curve_t curve, const uint64_t* P, const uint64_t* 
   if (int rc = gmsm_pair_device(curve, dP.p, dQ.p, n, dO.p, dW.p, nullptr)) return rc;
   CK(cudaMemcpy(out, dO.p, gb, cudaMemcpyDeviceToHost));
   return GMSM_OK;
+}
+
+// test hook: k_tower_op (tower_testops.cuh) over n host elements
+extern "C" int gmsm_test_tower_op(gmsm_curve_t curve, int op, const uint64_t* a, const uint64_t* b, uint64_t* out, size_t n) {
+  return with_pairing_field(curve, [&](auto p) {
+    using P = decltype(p);
+    int wa, wb, wo;
+    tower_op_sizes<P>(op, &wa, &wb, &wo);
+    if (wo == 0) return set_err(GMSM_EINVAL, "gmsm_test_tower_op: op %d is not an op of curve id %d", op, (int)curve);
+    if (n == 0) return (int)GMSM_OK;
+    if (n > 0xFFFFFFFFull || !a || (wb && !b) || !out) return set_err(GMSM_EINVAL, "gmsm_test_tower_op: invalid arguments");
+    if (int rc = use_device(default_device())) return rc;
+    const size_t e = sizeof(Fp2<P>);
+    DevBuf da, db, dout;
+    if (cudaMalloc(&da.p, n * wa * e) != cudaSuccess || cudaMalloc(&db.p, n * (wb ? wb : 1) * e) != cudaSuccess ||
+        cudaMalloc(&dout.p, n * wo * e) != cudaSuccess)
+      return set_err(GMSM_ENOMEM, "gmsm_test_tower_op: device allocation failed");
+    CK(cudaMemcpy(da.p, a, n * wa * e, cudaMemcpyHostToDevice));
+    if (wb) CK(cudaMemcpy(db.p, b, n * wb * e, cudaMemcpyHostToDevice));
+    k_tower_op<P><<<nblk(n, PAIRING_THREADS), PAIRING_THREADS>>>(op, da.as<Fp2<P>>(), db.as<Fp2<P>>(), dout.as<Fp2<P>>(), (uint32_t)n);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(out, dout.p, n * wo * e, cudaMemcpyDeviceToHost));
+    return (int)GMSM_OK;
+  });
 }

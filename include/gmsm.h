@@ -430,6 +430,40 @@ enum {
 };
 int gmsm_test_op(gmsm_curve_t curve, int op, const uint32_t* a, const uint32_t* b, uint32_t* out,
                  size_t n);
+/* the pairing towers of bn254 and bls12-381 (curve: the G1 id), element-wise on the device.  Widths in Fp2 units (an Fp2 is two
+ * Montgomery fp.Elements; E6 = 3, E12 = 6 in the GT layout, a line (R0, R1, R2) = 3, a G2 projective point (X, Y, Z) = 3, a G2
+ * affine point = 2, a G1 affine point = 1).  The line ops act on the curve's own sparse shape: positions 0, 3, 4 for bn254,
+ * 0, 1, 4 for bls12-381. */
+enum {
+  GMSM_TOWER_OP_E6_MUL = 0,                /* a: E6, b: E6 -> E6 */
+  GMSM_TOWER_OP_E6_INV = 1,                /* a: E6 -> E6 (0 -> 0) */
+  GMSM_TOWER_OP_E6_MUL_BY_01 = 2,          /* a: E6, b: c0, c1 -> E6 */
+  GMSM_TOWER_OP_E6_MUL_BY_1 = 3,           /* a: E6, b: c1 -> E6 */
+  GMSM_TOWER_OP_E6_MUL_BY_12 = 4,          /* a: E6, b: c1, c2 -> E6 */
+  GMSM_TOWER_OP_E12_MUL = 5,               /* a: E12, b: E12 -> E12 */
+  GMSM_TOWER_OP_E12_SQR = 6,               /* a: E12 -> E12, and so on for the one-operand E12 ops up to EXPT_HALF */
+  GMSM_TOWER_OP_E12_INV = 7,
+  GMSM_TOWER_OP_E12_CONJ = 8,
+  GMSM_TOWER_OP_E12_FROB1 = 9,
+  GMSM_TOWER_OP_E12_FROB2 = 10,
+  GMSM_TOWER_OP_E12_FROB3 = 11,
+  GMSM_TOWER_OP_E12_CYCLO_SQR = 12,
+  GMSM_TOWER_OP_E12_CYCLO_SQR_COMPRESSED = 13,
+  GMSM_TOWER_OP_E12_DECOMPRESS_KARABINA = 14,
+  GMSM_TOWER_OP_E12_EXPT = 15,
+  GMSM_TOWER_OP_E12_EXPT_HALF = 16,        /* bls12-381 only */
+  GMSM_TOWER_OP_E12_MUL_BY_LINE = 17,      /* a: E12, b: line -> E12 (MulBy034 / MulBy014) */
+  GMSM_TOWER_OP_LINE_BY_LINE = 18,         /* a: line, b: line -> 5 Fp2 (Mul034By034 / Mul014By014) */
+  GMSM_TOWER_OP_E12_MUL_BY_TWO_LINES = 19, /* a: E12, b: 5 Fp2 -> E12 (MulBy01234 / MulBy01245) */
+  GMSM_TOWER_OP_DOUBLE_STEP = 20,          /* a: G2 projective -> the doubled point, then its line (6) */
+  GMSM_TOWER_OP_ADD_MIXED_STEP = 21,       /* a: G2 projective, b: G2 affine -> the sum, then the line (6) */
+  GMSM_TOWER_OP_LINE_COMPUTE = 22,         /* a: G2 projective, b: G2 affine -> a unchanged, then the line (6) */
+  GMSM_TOWER_OP_FINAL_EXP = 23,            /* a: E12 -> FinalExponentiation(a) */
+  GMSM_TOWER_OP_MILLER_LOOP_ONE = 24       /* a: G1 affine, b: G2 affine, neither infinity -> MillerLoop of the pair */
+};
+/* a, b, out are HOST arrays of n elements at the op's widths (b unused by one-operand ops).  GMSM_EINVAL for another curve or an
+ * op the curve does not have. */
+int gmsm_test_tower_op(gmsm_curve_t curve, int op, const uint64_t* a, const uint64_t* b, uint64_t* out, size_t n);
 /* digits of partitionScalars (multiexp.go:709-803) as the device computes them: out[w*n + i] */
 int gmsm_test_digits(gmsm_curve_t curve, int c, const uint64_t* scalars, size_t n, uint32_t* out);
 

@@ -1,10 +1,12 @@
 // TEST INFRASTRUCTURE ONLY -- the pairing kernels (gnark-crypto_b200/csrc/pairing_kernels.cuh: k_miller_loop, k_gt_reduce,
 // k_gt_accumulate, k_final_exp) on the CPU, launched in the library's order (pairing_schedule, as pairing.cu's run_miller), for
-// bn254 (EMU_CURVE = 0) and bls12-381 (1).  tests/test_emu_pairing_cpu.py.
+// bn254 (EMU_CURVE = 0) and bls12-381 (1), and the tower test ops (tower_testops.cuh: k_tower_op).  tests/test_emu_pairing_cpu.py,
+// tests/test_tower_stress_cpu.py.
 #include <cstring>
 #include <vector>
 
 #include "pairing_kernels.cuh"
+#include "tower_testops.cuh"
 
 using namespace gmsm;
 
@@ -43,6 +45,16 @@ extern "C" void EMU_CAT(emu_miller_loop_, EMU_CURVE)(const void* pts, const void
       });
   emu_block_order = 0;
   std::memcpy(out, work.data() + pairing_acc_index(n, chunk), sizeof(G));
+}
+
+// out[i] = op(a[i], b[i]) for i < n (tower_testops.cuh, widths of tower_op_sizes); returns 0, or 1 for an op the curve does not have
+extern "C" int EMU_CAT(emu_tower_op_, EMU_CURVE)(int op, const void* a, const void* b, void* out, uint64_t n, unsigned threads) {
+  int wa, wb, wo;
+  tower_op_sizes<EmuP>(op, &wa, &wb, &wo);
+  if (wo == 0) return 1;
+  emu_launch(k_tower_op<EmuP>, dim3((unsigned)((n + threads - 1) / threads)), threads, op, reinterpret_cast<const Fp2<EmuP>*>(a),
+             reinterpret_cast<const Fp2<EmuP>*>(b), reinterpret_cast<Fp2<EmuP>*>(out), (uint32_t)n);
+  return 0;
 }
 
 // out = FinalExponentiation(z[0], z[1..k))
